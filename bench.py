@@ -2,7 +2,7 @@
 """
 bench.py — 16384-sample frames/s of the Wave-U-Net forward (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--precision fp32|bf16|auto]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--precision fp32|bf16|auto] [--dump-outputs DIR]
     python bench.py --impl reference ...        # the reference's CPU implementation of the path (host cores)
     python bench.py --mode train   [--batch 64] # SURVEY §8f N1 / configs[4]: fwd + bwd + Adam per step, grads all-reduced
     python bench.py --mode enhance              # configs[3]: 10 s clips through enhance_waveforms, 1024 frames/step sharded
@@ -79,7 +79,7 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tensor_tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json; bf16 sustained, kernels timed inside a long step)"}
-    return {"hbm_gbs": 6650.0, "tensor_tflops": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tensor_tflops": 989.0, "source": "H100 SXM data sheet (HBM3, dense bf16; a 700 W card)"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -237,31 +237,6 @@ def time_steps(fn, steps, warm=3):
     return e0.elapsed_time(e1) / steps
 
 
-def ncu_traffic(level: str, version: str):
-    """DRAM bytes per launch of one block from the committed ncu capture, but ONLY if that capture was taken from the build
-    that is running now (the summary CSV carries the library's source hash); otherwise (None, reason)."""
-    import csv
-    import glob
-    import re
-    m = re.search(r"src ([0-9a-f]+)", version)
-    cands = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_conv_tc_*summary.csv")))
-    if not m or not cands:
-        return None, "no ncu summary under profiles/"
-    path = cands[-1]
-    text = open(path).read()
-    if ("build " + m.group(1)) not in text:
-        return None, f"{os.path.basename(path)} was captured from a different build"
-    try:
-        rows = [r for r in csv.reader(text.splitlines()) if r and not r[0].startswith("#")]
-        hdr = rows[0]
-        for r in rows[1:]:
-            if r[0] == level:
-                return (float(r[hdr.index("dram_rd_MB")]) + float(r[hdr.index("dram_wr_MB")])) * 1e6, os.path.basename(path)
-    except Exception:  # noqa: BLE001
-        pass
-    return None, f"{level} not in {os.path.basename(path)}"
-
-
 def run_train(ctx):
     """SURVEY §8f row N1 / BASELINE.json configs[4]: one step = forward (train-mode BatchNorm) + MSE + backward + Adam on a
     batch of B frames per GPU (trainer/trainer.py:34-38, train.py:31-35); under torchrun the gradients are averaged over the
@@ -270,7 +245,7 @@ def run_train(ctx):
     from wave_u_net_for_speech_enhancement_b200 import Model, _lib
     from wave_u_net_for_speech_enhancement_b200.train_step import GradientBucket
     B = args.batch or 64
-    steps = min(args.steps, 20)
+    steps = args.steps
     model = Model(N_LAYERS, CH_INT)
     model.load_state_dict(st, strict=True)
     model = model.to(dev).train()
@@ -404,7 +379,7 @@ def run_enhance(ctx):
     args, rank, world, dev, dist, emit, st = (ctx[k] for k in ("args", "rank", "world", "dev", "dist", "emit", "st"))
     from wave_u_net_for_speech_enhancement_b200 import Model, _lib, enhance
     per_gpu = args.batch or 128
-    steps = min(args.steps, 20)
+    steps = args.steps
     clips_per_step = max(1, (per_gpu * world) // 10)
     rng = np.random.default_rng(7)
     clips = [(0.3 * rng.standard_normal(160000)).astype(np.float32) for _ in range(min(clips_per_step, 16))]
@@ -463,8 +438,12 @@ def main():
     ap.add_argument("--precision", default="auto", choices=["auto", "fp32", "bf16"])
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="forward mode: after the timed steps, write the output of the last timed step as DIR/y.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    if args.dump_outputs and args.mode != "forward":
+        ap.error("--dump-outputs is implemented for --mode forward")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -498,7 +477,7 @@ def main():
         return
 
     # --------------------------------------------------------------------------------------------
-    # B200 arm
+    # GPU arm
     # --------------------------------------------------------------------------------------------
     assert torch.cuda.is_available(), "bench.py needs a CUDA device (no CPU fallback on the product path)"
     torch.cuda.set_device(local_rank)
@@ -562,12 +541,18 @@ def main():
     barrier()
     if sampler:
         sampler.start()
+    y_last = None
     e0.record()
     for i in range(args.steps):
-        step(i)
+        y_last = step(i)                                       # a fresh output tensor per call: holding it costs nothing
     e1.record()
     torch.cuda.synchronize()
     ms_total = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0 and y_last is not None:
+        # [B, 1, T] float32 (16 MB at the default batch); the inputs are seeded, so two builds can be compared output for output
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "y.npy"), y_last.float().cpu().numpy())
+    del y_last
     # the timed region is tens of milliseconds; nvidia-smi samples every 100 ms. Keep issuing the identical step (untimed)
     # for ~1.2 s so that the clock / throttle record is taken under the same load.
     t_load = time.perf_counter()
@@ -620,7 +605,7 @@ def main():
     else:
         roof = {"bound": "tensor", "achieved": d["tflops"], "peak": peaks["tensor_tflops"], "unit": "TFLOP/s",
                 "frac": round(d["tflops"] / peaks["tensor_tflops"], 4)}
-    traffic, traffic_src = ncu_traffic(dname.split("+")[0], _lib.load().wunet_version().decode()) if (precision == "bf16" and B == 256) else (None, None)
+    traffic, traffic_src = None, "not measured (no DRAM counter capture of this build)"
     roof.update({"kernel": dname, "kernel_ms": d["ms"], "traffic": traffic, "traffic_source": traffic_src, "algorithmic_bytes": dbytes,
                  "algorithmic_flops": dflops, "peak_source": peaks["source"],
                  "net_frac": round(sum(l["roof_ms"] for l in levels) / sum(l["ms"] for l in levels), 4),
@@ -682,13 +667,13 @@ def main():
             lat["precision"] = precision
         extras["latency_b1"] = lat
         # BASELINE.json configs[1]: fp32 (<= 1e-4 path), batch 64. CUDA-core FFMA: its ceiling is the FFMA rate, not the
-        # tensor peak (148 SMs x 128 lanes x 2 flop x sm_max_mhz; theoretical, not driver-measured)
+        # tensor peak (H100 SXM: 132 SMs x 128 lanes x 2 flop x 1980 MHz boost clock; theoretical, not driver-measured)
         m32 = make("fp32")
         x64 = xs[0][:64].contiguous()
         with torch.no_grad():
             ms32 = time_steps(lambda: m32(x64), 10)
         flops64 = sum(f for _n, f, _b in block_table(64, 4))
-        ffma_peak = 148 * 128 * 2 * 1965e6
+        ffma_peak = 132 * 128 * 2 * 1980e6
         extras["fp32_config2"] = {"workload": "unet_basic forward fp32 (FFMA path, <= 1e-4 vs the reference), batch 64 x 16384 samples",
                                   "value": round(64 / ms32 * 1e3, 1), "unit": "frames/s", "ms_per_step": round(ms32, 4),
                                   "roofline": {"bound": "ffma", "achieved": round(flops64 / (ms32 * 1e-3) / 1e12, 2),
@@ -696,13 +681,13 @@ def main():
                                                "frac": round(flops64 / (ms32 * 1e-3) / ffma_peak, 4),
                                                "peak_source": "theoretical FFMA rate at sm_max_mhz (not driver-measured)"}}
         del m32
-        # the same <= 1e-4 contract on the tensor cores: split precision (bf16 hi + lo, three tcgen05 MMAs per product)
+        # the same <= 1e-4 contract on the tensor cores: split precision (bf16 hi + lo, three wgmma products per term)
         try:
             mtc = make("fp32_tc")
             with torch.no_grad():
                 ms_tc64 = time_steps(lambda: mtc(x64), 10)
                 ms_tc = time_steps(lambda: mtc(xs[0]), 10)
-            extras["fp32_tc"] = {"workload": "unet_basic forward, split-precision tcgen05 path (<= 1e-4 vs the reference)",
+            extras["fp32_tc"] = {"workload": "unet_basic forward, split-precision tensor-core path (<= 1e-4 vs the reference)",
                                  "batch64": {"value": round(64 / ms_tc64 * 1e3, 1), "unit": "frames/s", "ms_per_step": round(ms_tc64, 4)},
                                  f"batch{B}": {"value": round(B / ms_tc * 1e3, 1), "unit": "frames/s", "ms_per_step": round(ms_tc, 4)}}
             del mtc

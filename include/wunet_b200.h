@@ -1,5 +1,5 @@
 /*
- * wunet_b200.h — C ABI of the B200-native Wave-U-Net forward path.
+ * wunet_b200.h — C ABI of the H100-native Wave-U-Net forward path.
  *
  * This is the drop-in boundary for ONE hot path of haoxiangsnr/Wave-U-Net-for-Speech-Enhancement:
  * `Model.forward` (reference model/unet_basic.py:77-100) together with the parameter tree that
@@ -35,8 +35,8 @@ extern "C" {
 
 /* arithmetic of the convolution path */
 #define WUNET_PREC_FP32 0   /* fp32 operands, fp32 FFMA accumulate: parity <= 1e-4 vs reference (config 2) */
-#define WUNET_PREC_BF16 1   /* bf16 operands/activations, fp32 accumulate on tcgen05 tensor cores (config 3) */
-#define WUNET_PREC_FP32_TC 2 /* fp32-grade on the tensor cores: activations and weights split into bf16 high + low parts, three tcgen05
+#define WUNET_PREC_BF16 1   /* bf16 operands/activations, fp32 accumulate on wgmma tensor cores (config 3) */
+#define WUNET_PREC_FP32_TC 2 /* fp32-grade on the tensor cores: activations and weights split into bf16 high + low parts, three wgmma
                                MMAs per product (hi*hi + lo*hi + hi*lo, fp32 accumulate): <= 1e-4 vs the reference like WUNET_PREC_FP32 */
 
 typedef struct wunet_ctx wunet_ctx;
@@ -196,11 +196,11 @@ int wunet_train_backward_part(wunet_ctx *ctx, const float *x, const float *y, co
 /* Introspection for tests and tuning, host-only (needs no GPU, no context): the tiling the bf16 path would use for conv
  * block `block` (1 .. 2*n_layers; block 0 = first encoder runs on CUDA cores) at batch B, frame length T, on a device with
  * num_sms SMs. No reference counterpart. Writes 32 ints:
- *  [0] L  [1] Cin0  [2] Cin1  [3] Cout  [4] Npad  [5] N per CTA  [6] column splits  [7] TMEM column stride  [8] MT (128-row
+ *  [0] L  [1] Cin0  [2] Cin1  [3] Cout  [4] Npad  [5] N per CTA  [6] column splits  [7] accumulator column stride  [8] MT (128-row
  *  sub-tiles per tile)  [9] accumulator buffers  [10] packed frames  [11] frames per tile  [12] rows per packed frame
- *  [13] M tiles  [14] K chunks  [15] weights resident  [16] TMA-store epilogue  [17] input stages  [18] weight stages
+ *  [13] M tiles  [14] K chunks  [15] weights resident  [16] TMA-store epilogue (always 0)  [17] input stages  [18] weight stages
  *  [19] taps per weight stage  [20] weight stages per chunk  [21] input stage bytes  [22] weight stage bytes
- *  [23] TMA bytes per input chunk  [24] input rows used  [25] TMEM columns  [26] dynamic shared memory bytes
+ *  [23] TMA bytes per input chunk  [24] input rows used  [25] unused (0)  [26] dynamic shared memory bytes
  *  [27] threads per CTA  [28] CTAs per SM  [29] grid  [30] small (two-CTAs-per-SM) flavour  [31] tiles per frame */
 int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity);
 

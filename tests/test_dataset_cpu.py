@@ -1,10 +1,8 @@
 """Training-side data path (SURVEY §8f row N4): the native wav reader + aligned random crop against the reference's
 `dataset/waveform_dataset.py:56-67` / `util/utils.py:101-113`. CPU only. The wav files are written here with scipy / the
-stdlib; where `/root/reference` exists the UNCHANGED reference Dataset class is driven next to the drop-in (its `librosa.load`
-stubbed with a scipy reader that converts like soundfile does), with the same numpy seed."""
+stdlib; the items the UNCHANGED reference Dataset class gave for the same files and numpy seed (its `librosa.load` stubbed with a
+scipy reader that converts like soundfile does) are stored as golden digests."""
 import os
-import sys
-import types
 import wave
 
 import torch
@@ -16,7 +14,6 @@ import scipy.io.wavfile as wavfile
 from wave_u_net_for_speech_enhancement_b200 import _lib
 from wave_u_net_for_speech_enhancement_b200 import dataset as ds
 
-REF = "/root/reference"
 
 
 def soundfile_like(path):
@@ -131,35 +128,19 @@ def test_dataset_items_and_crops(tmp_path):
         ds.Dataset(lst, sample_length=30000)[0]                   # clip shorter than sample_length: the reference asserts too
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "dataset")), reason="reference checkout not present on this box")
-def test_dataset_matches_unchanged_reference_class(tmp_path, monkeypatch):
-    lst, _lines = _pair_files(tmp_path)
-    stub = types.ModuleType("librosa")
-    stub.load = lambda path, sr=None: soundfile_like(path)
-    monkeypatch.setitem(sys.modules, "librosa", stub)
-    for name in ("pesq", "pystoi", "pystoi.stoi"):
-        m = types.ModuleType(name)
-        m.pesq = m.stoi = lambda *a, **k: 0.0
-        monkeypatch.setitem(sys.modules, name, m)
-    sys.modules["pystoi"].stoi = sys.modules["pystoi.stoi"]
-    monkeypatch.syspath_prepend(REF)
-    for name in [k for k in sys.modules if k.split(".")[0] in ("util", "dataset")]:
-        monkeypatch.delitem(sys.modules, name)
-    import importlib
-    ref_ds = importlib.import_module("dataset.waveform_dataset")
-    try:
-        for mode in ("train", "validation"):
-            r = ref_ds.Dataset(lst, sample_length=16384, mode=mode)
-            o = ds.Dataset(lst, sample_length=16384, mode=mode)
-            np.random.seed(7)
-            want = [r[i] for i in range(len(r))]
-            np.random.seed(7)
-            got = [o[i] for i in range(len(o))]
-            for (wm, wc, wn), (gm, gc, gn) in zip(want, got):
-                assert wn == gn and wm.shape == gm.shape and np.array_equal(wm, gm) and np.array_equal(wc, gc)
-    finally:
-        for name in [k for k in sys.modules if k.split(".")[0] in ("util", "dataset")]:
-            sys.modules.pop(name, None)
+def test_dataset_matches_unchanged_reference_class(golden_dir, tmp_path):
+    """The reference's unchanged Dataset class (dataset/waveform_dataset.py, librosa.load as soundfile_like) gave the items
+    recorded in tests/golden/dataset_reference_items.json (oracle/gen_golden_boundary.py) for these files and np.random seed:
+    the drop-in must give the same names, shapes and bytes in both modes."""
+    import json
+    from oracle import boundary_common as bc
+    lst, _lines = bc.write_dataset_pairs(str(tmp_path))
+    want = json.load(open(os.path.join(golden_dir, "dataset_reference_items.json")))
+    for mode in ("train", "validation"):
+        o = ds.Dataset(lst, sample_length=16384, mode=mode)
+        np.random.seed(7)
+        got = [bc.item_digest(o[i]) for i in range(len(o))]
+        assert got == want[mode], mode
 
 
 @pytest.mark.parametrize("pcm", [False, True])

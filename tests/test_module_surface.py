@@ -116,7 +116,7 @@ def test_torch_training_path_matches_oracle_in_eval_semantics():
     assert np.abs(y - wo.COracle(n, ci).forward(st, x)).max() <= 1e-5
 
 
-def test_empty_batch_like_the_reference():
+def test_empty_batch_like_the_reference(golden_dir):
     """Zero frames: the reference's eval forward returns an empty [0, 1, T] tensor and still rejects a bad length; so does the
     drop-in, without touching the device (the C ABI itself takes B >= 1)."""
     m = Model(4, 8).eval()
@@ -125,15 +125,9 @@ def test_empty_batch_like_the_reference():
     assert m.forward_host(torch.zeros(0, 1, 256)).shape == (0, 1, 256)
     with pytest.raises(RuntimeError, match="not a multiple"):
         m(torch.zeros(0, 1, 100))
-    ref_root = "/root/reference"
-    if os.path.isdir(ref_root):                                   # live reference (this container only)
-        import sys
-        sys.path.insert(0, ref_root)
-        try:
-            from model.unet_basic import Model as RefModel
-            assert RefModel(4, 8).eval()(torch.zeros(0, 1, 256)).shape == y.shape
-        finally:
-            sys.path.remove(ref_root)
+    # what the reference module returned for the same call (recorded by oracle/gen_golden_boundary.py)
+    want = json.load(open(os.path.join(golden_dir, "reference_empty_batch.json")))
+    assert list(y.shape) == want["shape"] and str(y.dtype) == want["dtype"]
 
 
 def test_library_builds_and_exports_header_symbols():

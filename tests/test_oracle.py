@@ -119,7 +119,7 @@ def test_batch_independence():
 
 def test_bf16_arithmetic_model_sits_where_the_gpu_path_was_measured(golden_dir):
     """oracle/wunet_bf16_model.py restates the bf16 path's roundings; against the fp32 golden vectors it must show the
-    distance the CUDA path showed on the B200 (0.3-0.5 % of each level's range, ~6e-4 on the output), not more."""
+    distance the CUDA path is held to (test_parity_gpu.py: 0.8 % of each level's range, 2e-3 on the output), not more."""
     from oracle import wunet_bf16_model as wb
     g = np.load(os.path.join(golden_dir, "small_n4_c8.npz"))
     n, ci, T, B = int(g["n_layers"]), int(g["channels_interval"]), int(g["T"]), int(g["B"])

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu). The CUDA path is called through the C ABI
+"""GPU parity tests (pytest -m gpu, on an H100). The CUDA path is called through the C ABI
 (via the drop-in module's ctypes shim) and compared with the oracle and the committed golden vectors
 generated from the live reference module."""
 import os
@@ -40,8 +40,8 @@ def state_full():
 
 def test_extension_is_loaded_not_a_fallback():
     lib = _lib.load()
-    assert b"sm_100a" in lib.wunet_version()
-    assert torch.cuda.get_device_capability(0)[0] == 10
+    assert b"sm_90a" in lib.wunet_version()
+    assert torch.cuda.get_device_capability(0) == (9, 0)
 
 
 def test_fp32_small_config_all_levels(golden_dir):
@@ -139,7 +139,7 @@ def test_forward_host_matches_device_path(state_full):
     assert np.array_equal(yh.numpy(), run(m, x))
 
 
-# ---- bf16 / tcgen05 path (BASELINE.json configs[2]) -------------------------------------------------------
+# ---- bf16 tensor-core path (BASELINE.json configs[2]) -------------------------------------------------------
 # Every activation is stored in bf16 (8 mantissa bits: relative rounding 2^-9 = 0.2 %) and every conv uses bf16
 # operands with fp32 accumulation, so the per-level bound is relative to the level's dynamic range:
 BF16_LEVEL_REL = 8e-3       # max-abs(level error) / max-abs(level) ; measured 0.3-0.5 %
@@ -215,30 +215,13 @@ def test_bf16_config3_batch256_properties(state_full):
     assert err <= BF16_OUT_TOL
     perm = np.random.default_rng(1).permutation(B)
     assert np.array_equal(run(m, x[perm]), y[perm])
-    # batches >= 128 take the tuned tilings of wunet_tc.cu (kTuned), smaller ones the generic rules: the K-loop order, hence
-    # every output bit, must not depend on the tiling. (Batches below 64 frames take the packed-frame kernels instead of the
+    # the tiling depends on the batch (column splits, grids), the K-loop order, hence every output bit, must not. (Batches below
+    # 64 frames take the packed-frame kernels instead of the
     # dense GEMM for the blocks of at most 16 samples - different arithmetic for the folded interpolation, so they are compared
     # among themselves.)
     assert np.array_equal(run(m, x[:64]), y[:64])
     assert np.array_equal(run(m, x[:3]), run(m, x[:5])[:3])
     assert np.isfinite(y).all() and np.abs(y).max() < 1.0
-
-
-def test_bf16_head_only_kernel_is_bit_identical(state_full):
-    """WUNET_TC_HEADK=1 (opt-in, DESIGN.md): the last decoder block runs the head-only instantiation - both operand chunks
-    written by the producer warps from a TMA-fed shared-memory ring, straight-line head epilogue. Same arithmetic in the same
-    order as the default kernel: every output bit equal, at a batch that takes the tuned (two CTAs per SM) tiling."""
-    B = 128
-    x = wo.make_input(B, 16384, seed=1357)
-    y0 = run(bf16_model(12, 24, state_full), x)
-    os.environ["WUNET_TC_HEADK"] = "1"
-    try:
-        y1 = run(bf16_model(12, 24, state_full), x)
-    finally:
-        os.environ.pop("WUNET_TC_HEADK", None)
-    assert np.array_equal(y0, y1)
-    want = wo.COracle(12, 24).forward(state_full, x[[0, 63, 127]])
-    assert np.abs(y1[[0, 63, 127]] - want).max() <= BF16_OUT_TOL
 
 
 def test_bf16_large_ragged_batch_and_long_frames(state_full):
@@ -277,7 +260,7 @@ def test_bf16_forward_host_matches_device_path(state_full):
 
 
 # ---- fp32_tc: fp32-grade results on the tensor cores (bf16 hi + lo split, three MMAs per product) -----------------------
-# BASELINE.json north_star asks for tcgen05 AND <= 1e-4 on the same path: every fp32 parity case again, same tolerance.
+# The tensor cores AND <= 1e-4 on the same path: every fp32 parity case again, same tolerance.
 def test_fp32_tc_small_config_all_levels(golden_dir):
     g = np.load(os.path.join(golden_dir, "small_n4_c8.npz"))
     n, ci, T, B = int(g["n_layers"]), int(g["channels_interval"]), int(g["T"]), int(g["B"])
@@ -337,9 +320,9 @@ def test_fp32_tc_config2_batch64_edges_and_odd_lengths(golden_dir, state_full):
 
 
 # ---- row-pair / row-group forms of the narrow blocks (DESIGN.md 5.1): every switch position against the oracle ------------
-@pytest.mark.parametrize("pair,enc0_tc", [("0", "0"), ("1", "0"), ("2", "0"), ("3", "0"), ("0", "1")])
+@pytest.mark.parametrize("pair,enc0_tc", [("0", "0"), ("1", "0"), ("0", "1")])
 def test_bf16_row_pair_and_group_forms_vs_oracle(state_full, pair, enc0_tc, monkeypatch):
-    """WUNET_TC_PAIR bit 0 (block 1 over pairs of positions: the default), bit 1 (last block + head over pairs), WUNET_TC_ENC0=1
+    """WUNET_TC_PAIR bit 0 (block 1 over pairs of positions: the default; 0 = the plain block), WUNET_TC_ENC0=1
     (block 0 on the tensor cores over groups of 8 samples): the same operator, so the same bounds as the plain blocks hold - per
     block against the oracle's activations, on the output, with impulses at both frame edges (zero padding of the row-pair rows,
     end points of the upsampling) - and the benchmarked variant (last block not stored) gives the same output."""

@@ -1,7 +1,7 @@
 """A/B of a kernel-path switch of the bf16 path (environment variable read when the library creates a context, "0" = off):
 output difference and per-block times, plus the error of both against the fp32 path on a few frames.
 
-    timeout 120 python tools/ab_check.py WUNET_TC_TN        # taps-in-N kernel for enc1 / dec10 / dec11
+    timeout 120 python tools/ab_check.py WUNET_TC_GEMM      # dense GEMM over frames for the blocks of <= 16 samples
     timeout 120 python tools/ab_check.py WUNET_TC_MERGE     # merged decoder tail chunk
 """
 import os
@@ -15,7 +15,7 @@ import torch  # noqa: E402
 from wave_u_net_for_speech_enhancement_b200 import Model  # noqa: E402
 
 
-VAR = sys.argv[1] if len(sys.argv) > 1 else "WUNET_TC_TN"
+VAR = sys.argv[1] if len(sys.argv) > 1 else "WUNET_TC_GEMM"
 
 
 def run(on, B, reps=5, precision="bf16"):

@@ -1,8 +1,8 @@
-"""One configuration of the row-pair experiment (WUNET_TC_PAIR) on a B200: correctness against the C oracle and the default
+"""One configuration of the row-pair experiment (WUNET_TC_PAIR) on the GPU: correctness against the C oracle and the default
 path, per-block outputs of the two blocks it changes, and per-block times at batch 256. One process per configuration, so
 that a hang in an experimental kernel is contained by `timeout`:
 
-    timeout 120 python tools/pair_check.py <pair mask 0..3> [WUNET_TC_OVR string]
+    timeout 120 python tools/pair_check.py <pair mask 0..1> [WUNET_TC_OVR string]
 
 Prints one JSON line (also appended to gpurun_out/pair/results.jsonl)."""
 import json

@@ -1,4 +1,4 @@
-"""Per-block tiling sweep of the bf16 path (development tool, needs a B200).
+"""Per-block tiling sweep of the bf16 path (development tool, needs the GPU).
 
     python tools/sweep_levels.py --journal gpurun_out/sweep.jsonl [--blocks 7,8] [--batch 256]
 

@@ -1,4 +1,4 @@
-"""Development check of the bf16 tcgen05 path: per-level max error vs the golden vectors (GPU box)."""
+"""Development check of the bf16 tensor-core path: per-level max error vs the golden vectors (GPU box)."""
 import os, sys
 os.environ.setdefault("WUNET_TC_STORE_LAST", "1")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -27,7 +27,7 @@ def load() -> ctypes.CDLL:
     if not os.path.exists(SO_PATH):
         raise ImportError(
             f"{SO_PATH} is missing: build it with `python -m wave_u_net_for_speech_enhancement_b200.build` "
-            "(needs nvcc; sm_100a only). This package has no CPU / PyTorch fallback for the forward path.")
+            "(needs nvcc; sm_90a only). This package has no CPU / PyTorch fallback for the forward path.")
     lib = ctypes.CDLL(SO_PATH)
     vp, ci, cs = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
     lib.wunet_version.restype = ctypes.c_char_p

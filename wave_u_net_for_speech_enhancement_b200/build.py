@@ -1,4 +1,4 @@
-"""In-tree build of libwunet_b200.so (nvcc, sm_100a only). `python -m wave_u_net_for_speech_enhancement_b200.build`"""
+"""In-tree build of libwunet_b200.so (nvcc, sm_90a only). `python -m wave_u_net_for_speech_enhancement_b200.build`"""
 import os
 import shutil
 import subprocess
@@ -27,8 +27,8 @@ def is_stale() -> bool:
 
 
 def source_hash() -> str:
-    """sha1 over the CUDA sources and headers (12 hex digits): compiled into wunet_version() so that profiles/ captures can be
-    matched to the binary they were taken from (bench.py only quotes ncu traffic from a capture of the running build)."""
+    """sha1 over the CUDA sources and headers (12 hex digits): compiled into wunet_version() so that recorded measurements can be
+    matched to the binary they were taken from."""
     import hashlib
     h = hashlib.sha1()
     for s in SOURCES + HEADERS:
@@ -42,17 +42,15 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if out_so == SO and not force and not is_stale():
         return SO
     objs = []
-    common = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    common = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-DWUNET_BUILD", f'-DWUNET_SRC_HASH="{source_hash()}"']
     if verbose:
         common += ["-Xptxas", "-v"]
     if os.environ.get("WUNET_TC_TRACE"):
         common += ["-DWUNET_TC_TRACE"]
-    for macro in ("WUNET_WAIT_NS", "WUNET_WAIT_NS_MMA", "WUNET_OPERAND_FENCE"):    # development: mbarrier suspend-time hints (A/B builds, tools/gpu_lib_ab.sh, tools/lib_times.py)
+    for macro in ("WUNET_WAIT_NS",):                  # development: mbarrier suspend-time hint (A/B builds)
         if os.environ.get(macro):
             common += [f"-D{macro}={int(os.environ[macro])}"]
-    if os.environ.get("WUNET_TN_DEBUG"):
-        common += ["-DWUNET_TN_DEBUG"]                  # development: conv_tn_kernel instantiations with one role switched off
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     procs = []
     for s in SOURCES:
@@ -66,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
-    link = [nvcc_path(), "-shared", "-o", out_so] + objs + ["-cudart", "static"]
+    link = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", out_so] + objs + ["-cudart", "static"]
     subprocess.check_call(link)
     return out_so
 

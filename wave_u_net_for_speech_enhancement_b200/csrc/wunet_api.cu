@@ -52,7 +52,7 @@ struct wunet_ctx {
     float *out_w = nullptr, *out_b = nullptr;   // device copies [ci+1], [1]
     bool have_weights = false;
     int last_launches = 0;
-    TcState *tc = nullptr;             // bf16 / tcgen05 path state (packed weights, tensor maps)
+    TcState *tc = nullptr;             // bf16 / wgmma path state (packed weights, tensor maps)
     bool profile = false;              // record per-block events (wunet_profile_enable)
     std::vector<cudaEvent_t> ev;       // 2n+3 events
     int ev_recorded = 0;
@@ -179,7 +179,7 @@ extern "C" {
 #ifndef WUNET_SRC_HASH
 #define WUNET_SRC_HASH "unknown"
 #endif
-const char *wunet_version(void) { return "wunet_b200 0.2 (sm_100a; fp32 FFMA + bf16 tcgen05 paths; src " WUNET_SRC_HASH ")"; }
+const char *wunet_version(void) { return "wunet_b200 0.3 (sm_90a; fp32 FFMA + bf16 wgmma paths; src " WUNET_SRC_HASH ")"; }
 
 const char *wunet_last_error(void) { return g_err; }
 
@@ -268,14 +268,14 @@ int wunet_set_weights(wunet_ctx *c, const float *const *conv_w, const float *con
     }
     CUDA_TRY(cudaMemcpyAsync(c->out_w, out_w, (c->ci + 1) * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(c->out_b, out_b, sizeof(float), cudaMemcpyDeviceToDevice, st));
-    // bf16 / tcgen05 path: repack from the folded fp32 copies
+    // bf16 / wgmma path: repack from the folded fp32 copies
     {
         std::vector<TcBlockSrc> src(c->blocks.size());
         for (size_t i = 0; i < c->blocks.size(); ++i)
             src[i] = TcBlockSrc{c->blocks[i].cin, c->blocks[i].cout, c->blocks[i].k, conv_w[i], c->blocks[i].scale,
                                 c->blocks[i].shift};
         const int r = tc_set_weights(&c->tc, c->n, c->ci, src.data(), (int)src.size(), c->out_w, c->out_b, st);
-        if (r != 0) return fail(WUNET_ECUDA, "tcgen05 weight packing failed: %s", tc_error());
+        if (r != 0) return fail(WUNET_ECUDA, "tensor-core weight packing failed: %s", tc_error());
     }
     c->have_weights = true;
     return WUNET_OK;
@@ -314,7 +314,7 @@ int wunet_forward(wunet_ctx *c, const float *x, float *y, int B, int T, int prec
     if (precision != WUNET_PREC_BF16 && precision != WUNET_PREC_FP32_TC) return fail(WUNET_EINVAL, "unknown precision %d", precision);
     const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, precision == WUNET_PREC_FP32_TC ? 1 : 0);
     if (ev && r == 0) c->ev_recorded = 2 * c->n + 3;
-    if (r != 0) return fail(WUNET_ECUDA, "tcgen05 forward failed: %s", tc_error());
+    if (r != 0) return fail(WUNET_ECUDA, "tensor-core forward failed: %s", tc_error());
     c->last_launches = launches;
     return WUNET_OK;
 }
@@ -347,7 +347,7 @@ int wunet_forward_host(wunet_ctx *c, const float *x_host, float *y_host, int B, 
         if (!c->have_weights) return fail(WUNET_ESTATE, "wunet_forward_host called before wunet_set_weights");
         int launches = 0;
         if (tc_forward_host(c->tc, x_host, y_host, c->hx, c->hy, B, T, c->hws, c->hstream, &launches, precision == WUNET_PREC_FP32_TC ? 1 : 0) != 0)
-            return fail(WUNET_ECUDA, "tcgen05 host pipeline failed: %s", tc_error());
+            return fail(WUNET_ECUDA, "tensor-core host pipeline failed: %s", tc_error());
         c->last_launches = launches;
         return WUNET_OK;
     }

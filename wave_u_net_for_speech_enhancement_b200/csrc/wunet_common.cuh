@@ -1,4 +1,4 @@
-// wunet_common.cuh — shared host/device declarations of the B200 Wave-U-Net forward library.
+// wunet_common.cuh — shared host/device declarations of the H100 Wave-U-Net forward library.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

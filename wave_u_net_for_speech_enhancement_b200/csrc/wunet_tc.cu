@@ -1,4 +1,4 @@
-// wunet_tc.cu — bf16 tensor-core path of the Wave-U-Net forward for sm_100a (tcgen05 + TMEM + TMA).
+// wunet_tc.cu — bf16 tensor-core path of the Wave-U-Net forward for sm_90a (wgmma + TMA + mbarrier).
 //
 // Data layout in HBM: every activation is channels-last bf16, [B][L][C] ("NLC"), C = the reference's
 // channel count (24*m). A Conv1d tap shift is then a whole-row shift of the operand tile.
@@ -6,32 +6,28 @@
 // Each conv block (reference: [decimate | interpolate+cat] -> Conv1d -> BatchNorm1d(eval) -> LeakyReLU,
 // model/unet_basic.py:83-86, :93-96, :10-13, :23-26) is ONE kernel, an implicit GEMM
 //     D[position, cout] = sum_taps sum_cin  X[position + tap - pad, cin] * W[tap][cout, cin]
-// with M = 128*MT output positions per CTA (TMEM lanes), N = Cout (padded to 16) and the K loop running
-// over 64-channel chunks x taps:
-//   * the input tile (128*MT + K-1 rows x 64 channels, 128B-swizzled) is loaded ONCE per chunk by TMA;
+// with M = 128 output positions per CTA tile, N = Cout (padded to 16, split over CTAs beyond the register budget) and the
+// K loop running over 64-channel chunks x taps:
+//   * the input tile (128 + K-1 rows x 64 channels, 128B-swizzled) is loaded ONCE per chunk by TMA;
 //     out-of-range rows/channels are zero-filled by TMA = Conv1d zero padding, per frame;
-//     every tap reuses it through a UMMA shared-memory descriptor whose start address is advanced by
-//     tap*128 B (verified on hardware by tools/umma_probe.cu);
+//     every tap reuses it through a wgmma shared-memory descriptor whose start address is advanced by tap*128 B;
 //   * encoder decimation o[:, :, ::2] is a tensor map with a doubled row stride (no copy);
 //   * decoder: the K axis is [upsampled previous output | skip]. The skip half comes by TMA; the upsampled
 //     half (F.interpolate linear, align_corners=True, index math in fp32 like ATen) is produced by the producer
 //     warps straight into the swizzled operand tile — the interpolated/concatenated tensor never exists in HBM;
-//   * weights come by TMA, shared by the MT sub-tiles: either a ring of stages holding several taps of one [N x 64]
-//     chunk each (as many as fit: every stage handshake idles the tensor pipe), or — where the whole packed weight
-//     set of the block fits next to the input ring — loaded once per persistent CTA;
-//   * accumulators live in TMEM (MT x N fp32 columns, double-buffered when 2 MT N <= 512 so that the next tile's MMAs
-//     overlap this tile's epilogue); the epilogue warps read them with tcgen05.ld, apply the
-//     folded BatchNorm scale/shift and LeakyReLU(0.1), and store bf16 NLC rows; the last decoder block also
+//   * weights come by TMA: either a ring of stages holding several taps of one [N x 64] chunk each, or — where the whole
+//     packed weight set of the block fits next to the input ring — loaded once per persistent CTA;
+//   * accumulators are registers of the consumer warpgroups that issue the wgmma; after the K loop the same threads apply
+//     the folded BatchNorm scale/shift and LeakyReLU(0.1) and store bf16 NLC rows; the last decoder block also
 //     applies the 1x1 conv over [decoder out | raw input] and tanh (model/unet_basic.py:98-99) so its 24-channel
 //     output never reaches HBM.
 //   * frames shorter than 128 samples (the bottom of the U) are packed several per tile with their own halo
 //     rows; rows that straddle two frames are computed and discarded.
-// Warp roles: epilogue warps (TMEM lane quadrant = warp % 4), upsample-producer warps (decoder blocks), one TMA
-// warp, one MMA-issue warp (highest warp id). Two kernel flavours per block type: "large" (one CTA per SM, 8 epilogue
-// + 9 producer warps) and "small" (two CTAs per SM: 4 + 4 warps, half the shared memory and TMEM each), so that one
-// CTA's pipeline bubbles are filled by the other's MMAs. build_plan() chooses tile shapes, ring depths and the flavour
-// per block (rules + a small table of swept tilings for the reference architecture); DESIGN.md §5 has the role table and
-// the measured hardware facts the design rests on.
+// Warp roles: consumer warpgroups (wgmma + epilogue), upsample-producer warps (decoder blocks), one TMA warp. Two kernel
+// flavours per block type: "large" (one CTA per SM, two consumer warpgroups + 4 producer warps, up to 128 columns) and
+// "small" (two CTAs per SM: one consumer warpgroup + 4 producer warps, up to 64 columns, half the shared memory), so that
+// one CTA's pipeline bubbles are filled by the other's MMAs. build_plan() chooses tile shapes, ring depths and the flavour
+// per block.
 #include "wunet_tc.cuh"
 #include "wunet_common.cuh"
 
@@ -58,10 +54,12 @@ int tc_fail(const char *fmt, ...)
     return -1;
 }
 
-constexpr int kEpiWarpsLarge = 8;                 // "large" flavour: two epilogue warps per TMEM lane quadrant ...
-constexpr int kProducerWarpsLarge = 9;            // ... plus nine upsample-producer warps in decoder blocks (one item per thread at MT=4)
-constexpr int kEpiWarpsSmall = 4;                 // "small" flavour (two CTAs per SM): one epilogue warp per quadrant,
+constexpr int kEpiWarpsLarge = 8;                 // "large" flavour: two consumer warpgroups (one m64 half of the tile each) ...
+constexpr int kProducerWarpsLarge = 4;            // ... plus four upsample-producer warps in decoder blocks (one item per thread)
+constexpr int kEpiWarpsSmall = 4;                 // "small" flavour (two CTAs per SM): one consumer warpgroup (both m64 halves),
 constexpr int kProducerWarpsSmall = 4;            // four producer warps
+constexpr int kAccColsLarge = 128;                // accumulator columns per CTA: 64 fp32 registers per consumer thread in
+constexpr int kAccColsSmall = 64;                 // either flavour
 constexpr int kSmemLimitSmall = 113 * 1024;       // 2 x (dynamic + 1 KB reserved) <= 228 KB per SM
 constexpr int kMaxBStages = 8;
 constexpr int kSmemLimit = 227 * 1024;
@@ -78,16 +76,11 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, int count)
 {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
-// Waiting on an mbarrier phase. try_wait suspends the thread in hardware only for a short, system-defined time (~80 cycles
-// measured on B200), so a plain retry loop is a hot spin: in the round-2 ncu capture of the decoder blocks a quarter of all
-// issued instructions were YIELD / TRYWAIT / BRA of waiting roles, competing with the epilogue and producer warps for the
-// issue slots. With a suspend-time hint ptxas emits NANOSLEEP.SYNCS (sleep until the barrier's phase flips or the time is
-// up) instead. WUNET_WAIT_NS: hint for the producer / epilogue / TMA roles, WUNET_WAIT_NS_MMA: for the MMA issuer; 0 = no hint.
+// Waiting on an mbarrier phase. try_wait suspends the thread in hardware only for a short, system-defined time, so a plain
+// retry loop is a hot spin that competes with the working roles for issue slots. With a suspend-time hint ptxas emits a
+// sleep until the barrier's phase flips or the time is up. WUNET_WAIT_NS: hint in ns for every role; 0 = no hint.
 #ifndef WUNET_WAIT_NS
 #define WUNET_WAIT_NS 0
-#endif
-#ifndef WUNET_WAIT_NS_MMA
-#define WUNET_WAIT_NS_MMA 0
 #endif
 template <int NS>
 __device__ __forceinline__ void mbar_wait_ns(uint32_t bar, uint32_t parity)
@@ -104,20 +97,7 @@ __device__ __forceinline__ void mbar_wait_ns(uint32_t bar, uint32_t parity)
                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     } while (!ok);
 }
-// tcgen05.fence::after_thread_sync after the MMA issuer's waits for operand stages (a_full / b_full). Strictly the mbarrier wait
-// is the acquire the MMA needs there (the operands arrive through the async proxy or st.shared + fence.proxy.async; the tcgen05
-// fence is about tcgen05 operations of different threads and stays after acc_empty in any case). Measured in round 2: a build
-// without these fences (-DWUNET_OPERAND_FENCE=0) is bit-identical and not faster (profiles/r02_ab_operand_fence.txt), so they stay.
-#ifndef WUNET_OPERAND_FENCE
-#define WUNET_OPERAND_FENCE 1
-#endif
-#if WUNET_OPERAND_FENCE
-#define OPERAND_FENCE() asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory")
-#else
-#define OPERAND_FENCE() do { } while (0)
-#endif
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) { mbar_wait_ns<WUNET_WAIT_NS>(bar, parity); }
-__device__ __forceinline__ void mbar_wait_mma(uint32_t bar, uint32_t parity) { mbar_wait_ns<WUNET_WAIT_NS_MMA>(bar, parity); }
 __device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity)
 {
     uint32_t ok;
@@ -134,77 +114,30 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_n(uint32_t bar, uint32_t count)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2)
 {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// one lane of a fully-converged warp (the code around it stays warp-uniform, so descriptors live in uniform registers)
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\telect.sync rx|px, 0xffffffff;\n\tselp.b32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// UMMA shared-memory descriptor of a K-major, 128B-swizzled operand (8-row groups 1024 B apart), as (lo, hi) words:
-//   lo = (addr >> 4) | LBO(1) << 16,  hi = SBO(1024 >> 4) | version(1) << 14 | SWIZZLE_128B(2) << 29.
-// base_offset stays 0 for ANY start row: the swizzle acts on absolute shared-memory address bits (tools/umma_probe.cu).
-// hi is loop-invariant and lo = base + small offsets, so the issuing lane spends one uniform add per operand per MMA
-// (tools/umma_rate.cu: 40 cycles/MMA at N=32 instead of ~110 with 64-bit descriptor arithmetic in the loop).
-__device__ __forceinline__ void umma_bf16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc,
-                                               uint32_t accumulate)
+// wgmma (sm_90a): a warpgroup-wide asynchronous MMA whose operands come from shared memory through descriptors and whose
+// accumulators are registers of the issuing warpgroup.
+// Shared-memory descriptor of a K-major, 128B-swizzled operand (8-row groups 1024 B apart), as (lo, hi) words:
+//   lo = (addr >> 4) | LBO(1) << 16,  hi = SBO(1024 >> 4) | SWIZZLE_128B(1) << 30, base_offset 0.
+// The swizzle acts on absolute shared-memory address bits, so a start address advanced by whole 128-byte rows (the tap
+// shift of the implicit GEMM) or by 32 bytes (the next K16 step) addresses the TMA-written tile correctly.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 16] += A[64 x 16] * B[16 x 16]^T, bf16 operands, fp32 accumulators
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
 {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %5, 0;\n\tmov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}"
-        ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all MMAs of one tap: MT sub-tiles x nk K-steps. a_lo / b_lo are descriptor low words (16-byte units). Deliberately a
-// small rolled loop: the kernel's instruction footprint must stay cache-resident next to the epilogue / producer code.
-__device__ __forceinline__ void issue_tap(uint32_t d_col, int MT, uint32_t nstride, int nk, uint32_t a_lo, uint32_t b_lo,
-                                          uint32_t hi, uint32_t idesc, uint32_t acc_first)
-{
-#pragma unroll 1
-    for (int mt = 0; mt < MT; ++mt) {
-        umma_bf16_lohi(d_col, a_lo, b_lo, hi, idesc, acc_first);
-        if (nk > 1) umma_bf16_lohi(d_col, a_lo + 2, b_lo + 2, hi, idesc, 1u);
-        if (nk > 2) umma_bf16_lohi(d_col, a_lo + 4, b_lo + 4, hi, idesc, 1u);
-        if (nk > 3) umma_bf16_lohi(d_col, a_lo + 6, b_lo + 6, hi, idesc, 1u);
-        d_col += nstride;
-        a_lo += 128 * 8;                          // next 128-row sub-tile: 128 rows x 128 B = 1024 sixteen-byte units
-    }
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%8, %10};\n\tmov.b64 db, {%9, %10};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
 }
 __device__ __forceinline__ void st_shared_v4_if(uint32_t addr, const uint4 &v, bool pred)
 {
@@ -248,10 +181,10 @@ struct TcParams {
                                  // bit 6: merged tail chunk (MG kernels) / low-part data (split-precision kernels); bit 5 (split
                                  // precision): the position re-uses the operand stage of the position before it
     // N tiling
-    int Npad, Nh, Nstride;     // padded Cout, columns per CTA, TMEM column stride between sub-tile accumulators
+    int Npad, Nh, Nstride;     // padded Cout, columns per CTA, column stride between sub-tile accumulators
     // M tiling
     int MT, packed, S, FR, tiles_per_frame;
-    int m_tiles, nsplit, nacc; // M tiles in the problem, N halves, accumulator buffers in TMEM
+    int m_tiles, nsplit, nacc; // M tiles in the problem, N halves, accumulator buffers (1)
     int tile_begin, tile_end;  // tiles [begin, end) handled by this launch (sub-ranges = batch chunks of the host pipeline)
     int nops, R1, a_tx_bytes;  // TMA ops per A chunk, rows advanced per op, bytes per chunk
     int rows_used;             // smem rows the producers must fill (upsample path)
@@ -259,8 +192,8 @@ struct TcParams {
     int nb;                    // B ring depth
     int na;                    // A stages (1 or 2)
     int tg, ngroups;           // taps per weight stage, stages per chunk (= ceil(KS / tg))
-    int n_epi;                 // epilogue warps of this kernel flavour (slab count for bulk stores)
-    int bulk_store;            // 1: epilogue stages 32-row slabs in smem and writes them with cp.async.bulk (contiguous NLC rows)
+    int n_epi;                 // consumer warps of this kernel flavour
+    int bulk_store;            // always 0: the epilogue stores straight from the accumulator fragments
     int resident;              // 1: all weight tiles of the block stay in shared memory for the CTA's lifetime (no ring)
     uint32_t tmem_cols;
     // operands
@@ -306,7 +239,7 @@ __host__ __device__ inline SmemMap smem_map(const TcParams &p)
     m.b = p.na * p.a_stage_bytes;
     m.ss = m.b + p.nb * p.b_stage_bytes;
     m.stg = (m.ss + (uint32_t)p.Npad * 8 + 64 * 4 + 1023) & ~1023u;   // after scale/shift + head weights
-    m.ps = m.stg + (p.bulk_store ? (uint32_t)(p.n_epi * 2048) : 0u);     // one [32 rows x 32 ch] bf16 slab per epilogue warp
+    m.ps = m.stg;
     m.ps = (m.ps + 127) & ~127u;
     m.bars = m.ps + (uint32_t)p.ps_n * p.ps_bytes;                       // HD: ring of previous-level row windows
     m.bars = (m.bars + 15) & ~15u;
@@ -366,7 +299,7 @@ __device__ __forceinline__ ChunkInfo chunk_info(const TcParams &p, int c)
 // is bound by its operand reads, 32 + N/4 cycles) and the K loop shrinks; for the decoder the producers write the upsampled
 // half as [q0: 32 channels | q1: the same 32 channels] per 64-wide chunk and the fused head produces two samples per row.
 template <int KS, bool UPCAT, int EW, int PW, int MG, int SP = 0, int HD = 0, int PR = 0>
-__global__ void __launch_bounds__(64 + 32 * (EW + PW), EW == kEpiWarpsSmall ? 2 : 1)
+__global__ void __launch_bounds__(32 + 32 * (EW + PW), EW == kEpiWarpsSmall ? 2 : 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmO, const TcParams p)
 {
@@ -379,48 +312,35 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
     const SmemMap sm = smem_map(p);
     const uint32_t bars = base + sm.bars;
-    // barrier slots (8 B each): a_full[4] a_empty[4] b_full[8] b_empty[8] acc_full[2] acc_empty[2] | tmem slot
+    // barrier slots (8 B each): a_full[4] a_empty[4] b_full[8] b_empty[8] | 5 unused | a_tma[4] | p_full[8] p_empty[8]
     const uint32_t a_full = bars, a_empty = bars + 32, b_full = bars + 64, b_empty = bars + 64 + 8 * kMaxBStages;
-    const uint32_t acc_full = bars + 64 + 16 * kMaxBStages, acc_empty = acc_full + 16;
-    const uint32_t tmem_slot = acc_empty + 16;
-    const uint32_t a_tma = tmem_slot + 16;            // [4], MG = 1 kernels (merged tail chunk) only (smem_total reserves them)
+    const uint32_t a_tma = bars + 64 + 16 * kMaxBStages + 48;   // [4], MG = 1 kernels (merged tail chunk) only (smem_total reserves them)
     const uint32_t p_full = a_tma + 32, p_empty = a_tma + 96;   // [8] each, HD = 1 kernels only: ring of row windows (see the TMA role)
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(base_ptr + sm.bars + 64 + 16 * kMaxBStages + 32);
 
     // Programmatic dependent launch: let the next block's kernel be scheduled as our CTAs retire, so its prologue (barrier
-    // init, TMEM allocation, descriptor prefetch, resident weight preload) overlaps this kernel's tail.
+    // init, descriptor prefetch, resident weight preload) overlaps this kernel's tail.
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // warp roles. The scheduler of an SM sub-partition favours the highest warp id among eligible warps, so the two
-    // single-lane service warps (TMA, MMA issue) sit at the top: the MMA issuer must never queue behind epilogue math.
+    // warp roles: consumer warpgroups (wgmma + epilogue) first, so that they are aligned warpgroups, then the upsample producers
+    // (decoder blocks) and the TMA warp, the last warp of the launch shape (32 + 32 (EW + PW) threads).
     constexpr int kFirstProducer = kEpilogueWarps;
     constexpr int kTmaWarp = kEpilogueWarps + (UPCAT ? kProducerWarps : 0);
-    constexpr int kMmaWarp = kTmaWarp + 1;
     const int total_tiles = p.tile_end;
     const int first_tile = p.tile_begin + (int)blockIdx.x;
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
-        if (p.bulk_store) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
         for (int s = 0; s < 4; ++s) {
             mbar_init(a_full + 8 * s, HD != 0 ? kProducerWarps : (UPCAT ? 1 + kProducerWarps : 1));
-            mbar_init(a_empty + 8 * s, 1);
+            mbar_init(a_empty + 8 * s, kEpilogueWarps / 4);          // one arrival per consumer warpgroup
         }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(acc_full + 8 * s, 1);
-            mbar_init(acc_empty + 8 * s, kEpilogueWarps);
-        }
-        for (int s = 0; s < min(p.nb, kMaxBStages); ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 1); }
+        for (int s = 0; s < min(p.nb, kMaxBStages); ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, kEpilogueWarps / 4); }
         if (MG != 0 && p.mg)
             for (int s = 0; s < 4; ++s) mbar_init(a_tma + 8 * s, 1);
         if (HD != 0)
             for (int s = 0; s < 8; ++s) { mbar_init(p_full + 8 * s, 1); mbar_init(p_empty + 8 * s, kProducerWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == kMmaWarp) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(p.tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
     }
     {   // folded BatchNorm scale/shift of all output columns
         if (HD != 0) {
@@ -443,10 +363,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot_ptr;
     const bool pdl_early_weights = p.resident != 0;      // weights do not depend on the previous kernel's output
     if (!(warp == kTmaWarp && pdl_early_weights)) asm volatile("griddepcontrol.wait;" ::: "memory");
 
@@ -564,253 +481,130 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
             }
         }
-    } else if (warp == kMmaWarp) {
-        // ======================= MMA issuer =======================
-        // One elected lane runs the whole role (barrier waits included): every warp-level reconvergence between two weight
-        // stages costs tensor-pipe idle time, because the asynchronous MMA queue is only a few instructions deep.
-        if (elect_one()) {
-            int sa = 0, pa = 0, sb = 0, pb = 0, it = 0;
-            int tr1 = 0; (void)tr1;
-            int tr3 = 0; (void)tr3;
-            const uint32_t tile_bytes = (uint32_t)p.Nh * 128;
-            const uint32_t b_step = tile_bytes >> 4;
-            // descriptor words: hi = SBO(1024 B) | version 1 | SWIZZLE_128B, lo = (addr >> 4) | LBO(1)
-            const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-            if (p.resident) { mbar_wait_mma(b_full, 0); asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-            for (int tile = first_tile; tile < total_tiles; tile += gridDim.x, ++it) {
-                int b0, l0, n0;
-                tile_coords(tile, b0, l0, n0);
-                const int Nthis = min(p.Nh, p.Npad - n0);
-                // instruction descriptor: D=f32, A=B=bf16, both K-major, N>>3 at bit 17, M>>4 at bit 24
-                const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(Nthis >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-                const int buf = (p.nacc == 2) ? (it & 1) : 0;
-                const uint32_t use = (p.nacc == 2) ? (uint32_t)(it >> 1) : (uint32_t)it;
-                TRACE(1, tr1);
-                mbar_wait_mma(acc_empty + 8 * buf, (use & 1) ^ 1);
-                TRACE(1, tr1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t acc_col = tmem_base + buf * p.MT * p.Nstride;
-                for (int c = 0; c < p.nchunks; ++c) {
-                    const ChunkInfo mci = chunk_info<UPCAT, MG, SP>(p, c);
-                    const int nk = mci.nk;
-                    if (!(SP != 0 && mci.reuse)) {
-                        mbar_wait_mma(a_full + 8 * sa, pa);
-                        TRACE(1, tr1);
-                        OPERAND_FENCE();
-                    }
-                    const uint32_t a_base = base + sm.a + sa * p.a_stage_bytes;
-                    uint32_t a_lo = ((a_base >> 4) & 0x3FFFu) | (1u << 16);
-                    for (int g = 0; g < p.ngroups; ++g) {
-                        uint32_t b_base;
-                        if (p.resident) {
-                            b_base = base + sm.b + (uint32_t)(c * p.ngroups + g) * p.b_stage_bytes;
-                        } else {
-                            mbar_wait_mma(b_full + 8 * sb, pb);
-                            TRACE(1, tr1);
-                            OPERAND_FENCE();
-                            b_base = base + sm.b + sb * p.b_stage_bytes;
-                        }
-                        uint32_t b_lo = ((b_base >> 4) & 0x3FFFu) | (1u << 16);
-                        const int t_end = min(KS, (g + 1) * p.tg);
-#pragma unroll 1
-                        for (int t = g * p.tg; t < t_end; ++t) {
-                            TRACE(3, tr3);
-                            issue_tap(acc_col, p.MT, p.Nstride, nk, a_lo, b_lo, hi, idesc, (c | t) ? 1u : 0u);
-                            a_lo += 8;                                     // tap shift: +128 B
-                            b_lo += b_step;
-                        }
-                        if (!p.resident) umma_commit(b_empty + 8 * sb);
-                        if (++sb == p.nb) { sb = 0; pb ^= 1; }
-                    }
-                    // split precision: the next position may multiply the same operand stage with the low weight part
-                    if (!(SP != 0 && c + 1 < p.nchunks && chunk_info<UPCAT, MG, SP>(p, c + 1).reuse)) {
-                        umma_commit(a_empty + 8 * sa);
-                        if (++sa == p.na) { sa = 0; pa ^= 1; }
-                    }
-                }
-                umma_commit(acc_full + 8 * buf);
-            }
-        }
     } else if (warp < kEpilogueWarps) {
-        // ======================= epilogue warps (TMEM lane quadrant = warp % 4; two warps share a quadrant) ==========
-        const int q = warp & 3;
-        const int half = warp >> 2;                       // 0 .. kEpilogueWarps/4 - 1
-        constexpr int NSHARE = kEpilogueWarps / 4;        // warps sharing a quadrant
+        // ======================= consumer warpgroups: wgmma + epilogue =======================
+        // The tile's 128 rows are split into m64 blocks over the warpgroups (large flavour: one block each, small: two); every
+        // warpgroup runs the whole K loop for its rows with the accumulators in registers (n16 column blocks), releases each
+        // operand stage once its wgmma group has completed, then applies BatchNorm + LeakyReLU straight from the fragments.
+        // Fragment of m64nNk16 (f32): thread (warp wq, lane) holds rows 16 wq + lane / 4 (+8) and columns 2 (lane % 4) (+1) of
+        // every 8-column group.
+        constexpr int NWG = kEpilogueWarps / 4;
+        constexpr int MB = 2 / NWG;
+        constexpr int NB = (kEpilogueWarps == kEpiWarpsSmall ? kAccColsSmall : kAccColsLarge) / 16;
+        const int wg = warp >> 2, wq = warp & 3;
+        const bool wg_leader = (threadIdx.x & 127) == 0;
         const float2 *ss = reinterpret_cast<const float2 *>(base_ptr + sm.ss);
-        int it = 0;
-        int tr2 = 0; (void)tr2;
-        for (int tile = first_tile; tile < total_tiles; tile += gridDim.x, ++it) {
+        const float *hw = reinterpret_cast<const float *>(base_ptr + sm.ss) + 2 * p.Npad;   // head: [C+1] weights, bias
+        const uint32_t tile_bytes = (uint32_t)p.Nh * 128;
+        const uint32_t b_step = tile_bytes >> 4;
+        // descriptor words: hi = SBO(1024 B) | SWIZZLE_128B, lo = (addr >> 4) | LBO(1)
+        const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 30);
+        int sa = 0, pa = 0, sb = 0, pb = 0;
+        if (p.resident) mbar_wait(b_full, 0);
+        for (int tile = first_tile; tile < total_tiles; tile += gridDim.x) {
             int b0, l0, n0;
             tile_coords(tile, b0, l0, n0);
             const int Nthis = min(p.Nh, p.Npad - n0);
-            const int ncc = (Nthis + 31) >> 5;
-            const int buf = (p.nacc == 2) ? (it & 1) : 0;
-            const uint32_t use = (p.nacc == 2) ? (uint32_t)(it >> 1) : (uint32_t)it;
-            if (warp == 0 && lane == 0) TRACE(2, tr2);
-            // fused head: fetch the raw-input samples of this thread's rows before waiting for the accumulators
-            float xin0 = 0.f, xin1 = 0.f, xin2 = 0.f, xin3 = 0.f;     // scalars (not an array): they must stay in registers
-            if (PR != 0 && p.head && b0 < p.B) {
-                // row-pair mode: row l holds samples 2l and 2l+1 (MT <= 2: xin0/xin1 = the pair of sub-tile 0, xin2/xin3 of sub-tile 1)
-                const int lb = l0 + q * 32 + lane;
-                const float2 *xp2 = reinterpret_cast<const float2 *>(p.x + (size_t)b0 * p.T) + lb;
-                if (lb < p.L) { const float2 v2 = __ldg(xp2); xin0 = v2.x; xin1 = v2.y; }
-                if (p.MT > 1 && lb + 128 < p.L) { const float2 v2 = __ldg(xp2 + 128); xin2 = v2.x; xin3 = v2.y; }
-            } else
-            if (p.head && b0 < p.B) {
-                const float *xp = p.x + (size_t)b0 * p.T + l0 + q * 32 + lane;
-                const int lb = l0 + q * 32 + lane;
-                if (lb < p.L) xin0 = __ldg(xp);
-                if (p.MT > 1 && lb + 128 < p.L) xin1 = __ldg(xp + 128);
-                if (p.MT > 2 && lb + 256 < p.L) xin2 = __ldg(xp + 256);
-                if (p.MT > 3 && lb + 384 < p.L) xin3 = __ldg(xp + 384);
-            }
-            mbar_wait(acc_full + 8 * buf, use & 1);
-            if (warp == 0 && lane == 0) TRACE(2, tr2);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t acc_col = buf * p.MT * p.Nstride;
-            if (HD != 0) {
-                // head-only epilogue: BatchNorm + LeakyReLU of the (<= 32) columns of this thread's row, then
-                // cat([o, input], 1) -> Conv1d(C+1 -> 1, k=1) -> Tanh (model/unet_basic.py:98-99), accumulated in column order like
-                // the generic path. No bf16 conversion, no store of the block's activations, parameters as one LDS.128 per column.
-                const float4 *hp = reinterpret_cast<const float4 *>(base_ptr + sm.ss);
-                const float hbias = hp[0].w, hwin = hp[1].w;
+            const int nblk = Nthis >> 4;
+            float acc[MB][NB][8];
+#pragma unroll
+            for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+                for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) acc[mb][nb][j] = 0.f;
+            for (int c = 0; c < p.nchunks; ++c) {
+                const ChunkInfo mci = chunk_info<UPCAT, MG, SP>(p, c);
+                const int nk = mci.nk;
+                if (!(SP != 0 && mci.reuse)) mbar_wait(a_full + 8 * sa, pa);
+                const uint32_t a_base = base + sm.a + sa * p.a_stage_bytes + (uint32_t)(wg * MB * 64 * 128);
+                const uint32_t a_lo0 = ((a_base >> 4) & 0x3FFFu) | (1u << 16);
+                for (int g = 0; g < p.ngroups; ++g) {
+                    uint32_t b_base;
+                    if (p.resident) {
+                        b_base = base + sm.b + (uint32_t)(c * p.ngroups + g) * p.b_stage_bytes;
+                    } else {
+                        mbar_wait(b_full + 8 * sb, pb);
+                        b_base = base + sm.b + sb * p.b_stage_bytes;
+                    }
+                    const uint32_t b_lo0 = ((b_base >> 4) & 0x3FFFu) | (1u << 16);
+                    const int t0 = g * p.tg, t_end = min(KS, (g + 1) * p.tg);
+                    wgmma_fence();
 #pragma unroll 1
-                for (int mt = 0; mt < p.MT; ++mt) {
-                    const int l = l0 + mt * 128 + q * 32 + lane;
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc_col + (uint32_t)(mt * p.Nstride);
-                    float hacc = hbias;
+                    for (int t = t0; t < t_end; ++t) {
+                        const uint32_t a_t = a_lo0 + (uint32_t)t * 8u;                 // tap shift: +128 B
+                        const uint32_t b_t = b_lo0 + (uint32_t)(t - t0) * b_step;
 #pragma unroll
-                    for (int h16 = 0; h16 < 2; ++h16) {
-                        if (16 * h16 < p.Cout) {                                   // warp-uniform
-                            uint32_t v[16];
-                            tmem_ld16(taddr + 16 * h16, v);
+                        for (int k = 0; k < 4; ++k) {
+                            if (k >= nk) break;
 #pragma unroll
-                            for (int g8 = 0; g8 < 2; ++g8) {
-                                if (16 * h16 + 8 * g8 < p.Cout) {                  // warp-uniform; columns past Cout carry zero weights
+                            for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
-                                    for (int j = 0; j < 8; ++j) {
-                                        const float4 c4 = hp[16 * h16 + 8 * g8 + j];
-                                        hacc = fmaf(c4.z, lrelu(fmaf(__uint_as_float(v[8 * g8 + j]), c4.x, c4.y)), hacc);
-                                    }
+                                for (int nb = 0; nb < NB; ++nb)
+                                    if (nb < nblk) wgmma_n16(acc[mb][nb], a_t + (uint32_t)(mb * 512 + 2 * k), b_t + (uint32_t)(nb * 128 + 2 * k), hi);
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait0();
+                    if (!p.resident) {
+                        if (wg_leader) mbar_arrive(b_empty + 8 * sb);
+                        if (++sb == p.nb) { sb = 0; pb ^= 1; }
+                    }
+                }
+                // split precision: the next position may multiply the same operand stage with the low weight part
+                if (!(SP != 0 && c + 1 < p.nchunks && chunk_info<UPCAT, MG, SP>(p, c + 1).reuse)) {
+                    if (wg_leader) mbar_arrive(a_empty + 8 * sa);
+                    if (++sa == p.na) { sa = 0; pa ^= 1; }
+                }
+            }
+            // epilogue
+#pragma unroll
+            for (int mb = 0; mb < MB; ++mb) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = (wg * MB + mb) * 64 + 16 * wq + (lane >> 2) + 8 * h;
+                    int bb, l;
+                    if (p.packed) { const int f = row / p.S; bb = b0 + f; l = row - f * p.S; if (f >= p.FR) l = p.L; }
+                    else { bb = b0; l = l0 + row; }
+                    const bool valid = (bb < p.B) && (l < p.L);
+                    float hsum = 0.f;
+#pragma unroll
+                    for (int nb = 0; nb < NB; ++nb) {
+                        if (nb >= nblk) break;
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = nb * 16 + 8 * e + 2 * (lane & 3);            // column inside this CTA's N range
+                            const float4 s2 = *reinterpret_cast<const float4 *>(&ss[n0 + col]);
+                            const float f0 = lrelu(fmaf(acc[mb][nb][4 * e + 2 * h], s2.x, s2.y));
+                            const float f1 = lrelu(fmaf(acc[mb][nb][4 * e + 2 * h + 1], s2.z, s2.w));
+                            const bool col_ok = n0 + col < p.Cout;                        // Cout is even: both columns or none
+                            if (p.out != nullptr && valid && col_ok) {
+                                if (SP != 0) {
+                                    // split precision: the row holds [hi(Cout) | lo(Cout)]; lo = bf16(v - hi)
+                                    __nv_bfloat16 *orow = p.out + ((size_t)bb * p.L + l) * (2 * p.Cout) + n0 + col;
+                                    *reinterpret_cast<uint32_t *>(orow) = pack_bf16(f0, f1);
+                                    *reinterpret_cast<uint32_t *>(orow + p.Cout) =
+                                        pack_bf16(f0 - __bfloat162float(__float2bfloat16_rn(f0)), f1 - __bfloat162float(__float2bfloat16_rn(f1)));
+                                } else {
+                                    *reinterpret_cast<uint32_t *>(p.out + ((size_t)bb * p.L + l) * p.Cout + n0 + col) = pack_bf16(f0, f1);
                                 }
                             }
+                            if (p.head && col_ok) hsum = fmaf(hw[col + 1], f1, fmaf(hw[col], f0, hsum));
                         }
                     }
-                    if (b0 < p.B && l < p.L) {
-                        hacc = fmaf(hwin, mt == 0 ? xin0 : (mt == 1 ? xin1 : (mt == 2 ? xin2 : xin3)), hacc);
-                        p.y[(size_t)b0 * p.T + l] = tanh_fast(hacc);
-                    }
-                }
-            } else {
-            // Work items (mt, 32-column chunk) are dealt round-robin to the warps sharing a quadrant. One rolled code path
-            // serves the three store flavours (TMA-store slab, direct row stores, fused head): 16 accumulator columns are
-            // read per tcgen05.ld, converted 8 at a time.
-            uint8_t *slab = base_ptr + sm.stg + (uint32_t)warp * 2048u;
-            const uint32_t slab_s = smem_u32(slab);
-            uint8_t *srow = slab + lane * 64;
-            const int sw = (lane >> 1) & 3;
-            const float *hw = reinterpret_cast<const float *>(base_ptr + sm.ss) + 2 * p.Npad;   // head: [C+1] weights, bias
-            int turn = 0;
-#pragma unroll 1
-            for (int mt = 0; mt < p.MT; ++mt) {
-                const int row = mt * 128 + q * 32 + lane;
-                int bb, l;
-                if (p.packed) { const int f = row / p.S; bb = b0 + f; l = row - f * p.S; if (f >= p.FR) l = p.L; }
-                else { bb = b0; l = l0 + row; }
-                const bool valid = (bb < p.B) && (l < p.L);
-                const int hc = PR != 0 ? p.Cout >> 1 : p.Cout;
-                float hacc = p.head ? hw[hc + 1] : 0.f;
-                float haccb = hacc;                               // row-pair mode: the second sample of the row (columns hc .. 2 hc - 1)
-                bool did = false;                                 // this warp converted the row's (single) chunk
-#pragma unroll 1
-                for (int cc = 0; cc < ncc; ++cc) {
-                    if (NSHARE > 1) { const bool mine = (turn == half); turn = (turn + 1 == NSHARE) ? 0 : turn + 1; if (!mine) continue; }
-                    did = true;
-                    const int colbase = cc * 32;
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc_col + (uint32_t)(mt * p.Nstride + colbase);
-#pragma unroll 1
-                    for (int h16 = 0; h16 < 2; ++h16) {
-                        if (colbase + 16 * h16 >= Nthis) break;
-                        uint32_t v[16];
-                        tmem_ld16(taddr + 16 * h16, v);
-                        if (p.bulk_store && h16 == 0) {                   // slab free again? (previous TMA store has read it)
-                            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                            __syncwarp();
-                        }
-#pragma unroll
-                        for (int g8 = 0; g8 < 2; ++g8) {
-                            const int col = colbase + 16 * h16 + 8 * g8;       // column inside this CTA's N range
-                            float f[8];
-#pragma unroll
-                            for (int j = 0; j < 8; j += 2) {
-                                const float4 s2 = (col + j < Nthis) ? *reinterpret_cast<const float4 *>(&ss[n0 + col + j])
-                                                                    : make_float4(0.f, 0.f, 0.f, 0.f);
-                                f[j] = lrelu(fmaf(__uint_as_float(v[8 * g8 + j]), s2.x, s2.y));
-                                f[j + 1] = lrelu(fmaf(__uint_as_float(v[8 * g8 + j + 1]), s2.z, s2.w));
-                            }
-                            const uint4 o = make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-                            const bool col_ok = col < Nthis && n0 + col < p.Cout;
-                            if (p.bulk_store) {
-                                if (col_ok) *reinterpret_cast<uint4 *>(srow + (((2 * h16 + g8) ^ sw) << 4)) = o;
-                            } else if (SP != 0 && p.out != nullptr && valid && col_ok) {
-                                // split precision: the row holds [hi(Cout) | lo(Cout)]; lo = bf16(v - hi)
-                                float g[8];
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) g[j] = f[j] - __bfloat162float(__float2bfloat16_rn(f[j]));
-                                __nv_bfloat16 *orow = p.out + ((size_t)bb * p.L + l) * (2 * p.Cout) + n0 + col;
-                                *reinterpret_cast<uint4 *>(orow) = o;
-                                *reinterpret_cast<uint4 *>(orow + p.Cout) =
-                                    make_uint4(pack_bf16(g[0], g[1]), pack_bf16(g[2], g[3]), pack_bf16(g[4], g[5]), pack_bf16(g[6], g[7]));
-                            } else if (SP == 0 && p.out != nullptr && valid && col_ok) {
-                                *reinterpret_cast<uint4 *>(p.out + ((size_t)bb * p.L + l) * p.Cout + n0 + col) = o;
-                            }
-                            if (PR != 0 && p.head) {
-                                // hc % 8 == 0: a group of 8 columns belongs to one of the two samples
-                                if (col < hc) {
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) hacc = fmaf(hw[col + j], f[j], hacc);
-                                } else if (col < p.Cout) {
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) haccb = fmaf(hw[col - hc + j], f[j], haccb);
-                                }
-                            } else
-                            if (p.head) {
-#pragma unroll
-                                for (int j = 0; j < 8; ++j)
-                                    if (col + j < p.Cout) hacc = fmaf(hw[col + j], f[j], hacc);
-                            }
+                    if (p.head) {
+                        // cat([o, input], 1) -> Conv1d(C+1 -> 1, k=1) -> Tanh   (model/unet_basic.py:98-99); the four threads of a
+                        // row hold interleaved column pairs
+                        hsum += __shfl_xor_sync(0xffffffffu, hsum, 1);
+                        hsum += __shfl_xor_sync(0xffffffffu, hsum, 2);
+                        if (valid && (lane & 3) == 0) {
+                            const float hacc = fmaf(hw[p.Cout], __ldg(p.x + (size_t)bb * p.T + l), hw[p.Cout + 1] + hsum);
+                            p.y[(size_t)bb * p.T + l] = tanh_fast(hacc);
                         }
                     }
-                    if (p.bulk_store) {
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                        __syncwarp();
-                        if (lane == 0) {
-                            const int grow = b0 * p.L + l0 + mt * 128 + q * 32;       // row of the [B*L][Cout] view
-                            asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                                         ::"l"(reinterpret_cast<uint64_t>(&tmO)), "r"(slab_s), "r"(colbase), "r"(grow) : "memory");
-                            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                        }
-                    }
-                }
-                if (PR != 0 && p.head && valid) {
-                    // row-pair mode (one epilogue warp per quadrant: this warp converted every column of the row): two samples
-                    hacc = fmaf(hw[hc], mt == 0 ? xin0 : xin2, hacc);
-                    haccb = fmaf(hw[hc], mt == 0 ? xin1 : xin3, haccb);
-                    *reinterpret_cast<float2 *>(p.y + (size_t)bb * p.T + 2 * l) = make_float2(tanh_fast(hacc), tanh_fast(haccb));
-                } else
-                if (p.head && valid && did) {
-                    // cat([o, input], 1) -> Conv1d(C+1 -> 1, k=1) -> Tanh   (model/unet_basic.py:98-99); Cout <= 32: one chunk
-                    hacc = fmaf(hw[p.Cout], mt == 0 ? xin0 : (mt == 1 ? xin1 : (mt == 2 ? xin2 : xin3)), hacc);
-                    p.y[(size_t)bb * p.T + l] = tanh_fast(hacc);
                 }
             }
-            }
-            // accumulator buffer drained: hand it back to the MMA warp
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty + 8 * buf);
         }
-        if (p.bulk_store && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     } else if (UPCAT) {
         // ======================= upsample producers (decoder) =======================
         // F.interpolate(scale_factor=2, mode="linear", align_corners=True) of the previous block's output, written straight
@@ -1022,7 +816,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     // Row-pair instantiation: ALL upsampled chunks of the tile (K-loop positions 0 .. nchunks0 - 1, consecutive ring
                     // stages) are produced in ONE phase - one round of items over the producer threads, one fence, one hand-off. (Its
                     // first version produced them chunk by chunk: two phases per tile made the block 25 % slower than the plain form
-                    // although it issues half the MMAs, profiles/r02_row_pair_ab.txt.)
+                    // although it issues half the MMAs.)
                     if (c > 0) continue;
                     const int nup = p.nchunks0;
                     if (!pref) fetch(b0, l0, 0, pt);
@@ -1272,401 +1066,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == kMmaWarp) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols));
-}
-
-// -------------------------------------------------------------------------------------------------
-// "taps in N" kernel for the shallow, long blocks (Cout <= 48: enc1, dec10, dec11 of the reference architecture)
-// -------------------------------------------------------------------------------------------------
-// For N = Cout < 128 the M=128 MMA is bound by its shared-memory operand reads (32 + N/4 cycles, tools/umma_rate.cu): every
-// tap re-reads the same 4 KB A slab. Here G = 5 taps are folded into the N axis instead,
-//     D'[row, (t', co)] = sum_cin X[row, cin] * W[5g + t'][co, cin]        (one MMA of N' = 5 Cp columns per K16 step),
-// so the A slab is read once per 5 taps (dec11: 64 cycles instead of 5 x 40, dec10 / enc1: 120 instead of 5 x 44), and the
-// tap sum moves to the epilogue as a shifted sum over rows = TMEM lanes,
-//     out[l] = sum_t' D'[row(l) + t', t'],
-// done with warp shuffles (Horner: acc = D'[.,4]; acc = shfl_down(acc) + D'[.,3]; ...). A warp only reaches the 32 lanes of its
-// TMEM quadrant, so the operand tile is laid out in BLOCKS of 32 rows that overlap by 4 positions (block k holds positions
-// l0 - PAD + 28 k ... + 31): every quadrant then yields 28 complete output rows without any cross-warp exchange, at the price
-// of 12.5 % redundant MMA rows. A 15-tap encoder block runs its three tap groups as three K "chunks" (same channels, operand
-// rows shifted by 5 g positions, weight slot g). Everything else (TMA zero fill = conv padding, decimated / skip tensor maps,
-// upsample producers writing the swizzled operand, resident weights, double-buffered accumulators, fused head) is as in
-// conv_tc_kernel.
-struct TnParams {
-    int B, L, T, Cout, Cp, Npad, Nstride;      // Cp = column pitch of a tap inside N' (Cout rounded up to 8), Npad = N' padded to 16
-    int Cin0, Cin1;                            // decoder: upsampled / skip channels; encoder: Cin0 = Cin
-    int MT, tile_rows, tiles_per_frame;        // tile_rows = 112 MT output positions per tile
-    int tile_begin, tile_end;
-    int nchunks, na;                           // K chunks per tile, operand ring depth
-    unsigned char c_up[8], c_ch[8], c_nk[8], c_slot[8], c_row[8];   // per chunk: producer-written?, 64-channel chunk index inside its
-                                               // segment, K16 steps, weight slot, extra operand row offset (tap group * 5)
-    int pad;                                   // (KS - 1) / 2
-    int wpg, npg;                              // producer warps per group, groups (each group owns every npg-th tile)
-    int ntma, nup_items;                       // TMA-loaded chunks per tile; producer items per tile (all upsampled chunks)
-    uint32_t a_stage_bytes, a_sub_bytes, w_tile_bytes, tmem_cols;   // stage = all chunks of a tile, one sub-buffer (MT x 16 KB) each
-    const __nv_bfloat16 *prev;                 // decoder: previous block output [B][L/2][Cin0]
-    int Lin;
-    float up_scale;
-    const float2 *ss;                          // [Cout] folded BatchNorm (scale, shift)
-    __nv_bfloat16 *out;                        // [B][L][Cout] or nullptr (fused head without the debug store)
-    int head;
-    const float *x;
-    float *y;
-    const float *head_w, *head_b;
-    int dbg;                                   // development (WUNET_TN_DBG, -DWUNET_TN_DEBUG builds): selects a conv_tn_kernel<.., DBG> instantiation with one role
-                                               // switched off: 1 no tcgen05.ld, 2 no shuffles, 4 no stores, 8 no MMAs, 16 no TMA loads, 32 no producer work
-};
-struct TnSmem { uint32_t a, w, ss, bars; };
-__host__ __device__ inline TnSmem tn_smem_map(const TnParams &p)
-{
-    TnSmem m;
-    m.a = 0;
-    m.w = p.na * p.a_stage_bytes;
-    m.ss = m.w + p.nchunks * p.w_tile_bytes;
-    m.bars = (m.ss + (uint32_t)p.Cout * 8 + 64 * 4 + 15) & ~15u;
-    return m;
-}
-inline size_t tn_smem_total(const TnParams &p) { return tn_smem_map(p).bars + 8 * (8 + 8 + 1 + 2 + 2) + 16 + 1024; }   // barrier slots sized for 8 stages
-
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, uint32_t (&v)[8])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr));
-}
-
-template <bool UPCAT, int DBG>
-__global__ void __launch_bounds__(64 + 32 * (kEpiWarpsLarge + (UPCAT ? kProducerWarpsLarge : 0)), 1)
-conv_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TnParams p)
-{
-    constexpr int EW = kEpiWarpsLarge, PW = UPCAT ? kProducerWarpsLarge : 0;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const TnSmem sm = tn_smem_map(p);
-    const uint32_t bars = base + sm.bars;
-    // barrier slots (8 B each): a_full[8] a_empty[8] w_full[1] acc_full[2] acc_empty[2] | tmem slot
-    const uint32_t a_full = bars, a_empty = bars + 64, w_full = bars + 128, acc_full = bars + 136, acc_empty = bars + 152;
-    const uint32_t tmem_slot = bars + 168;
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(base_ptr + sm.bars + 168);
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr int kFirstProducer = EW, kTmaWarp = EW + PW, kMmaWarp = kTmaWarp + 1;
-    const int total_tiles = p.tile_end;
-    const int first_tile = p.tile_begin + (int)blockIdx.x;
-    if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
-        for (int s = 0; s < 8; ++s) {
-            mbar_init(a_full + 8 * s, (UPCAT && p.nup_items > 0) ? 1 + p.wpg : 1);
-            mbar_init(a_empty + 8 * s, 1);
-        }
-        mbar_init(w_full, 1);
-        for (int s = 0; s < 2; ++s) { mbar_init(acc_full + 8 * s, 1); mbar_init(acc_empty + 8 * s, EW); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == kMmaWarp) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(p.tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    {
-        float2 *ss = reinterpret_cast<float2 *>(base_ptr + sm.ss);
-        for (int i = threadIdx.x; i < p.Cout; i += blockDim.x) ss[i] = p.ss[i];
-        if (p.head) {
-            float *hw = reinterpret_cast<float *>(base_ptr + sm.ss) + 2 * p.Cout;
-            if ((int)threadIdx.x <= p.Cout) hw[threadIdx.x] = p.head_w[threadIdx.x];
-            if ((int)threadIdx.x == p.Cout + 1) hw[threadIdx.x] = p.head_b[0];
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot_ptr;
-    if (warp != kTmaWarp) asm volatile("griddepcontrol.wait;" ::: "memory");
-
-    auto tile_coords = [&](int tile, int &b0, int &l0) {
-        b0 = tile / p.tiles_per_frame;
-        l0 = (tile - b0 * p.tiles_per_frame) * p.tile_rows;
-    };
-    const int nblk = 4 * p.MT;                               // 32-row operand blocks per tile
-
-    if (warp == kTmaWarp) {
-        if (lane == 0) {
-            // the block's whole weight set: one [Npad x 64] tile per K chunk, loaded once per CTA (independent of the previous kernel)
-            mbar_expect_tx(w_full, (uint32_t)p.nchunks * (uint32_t)p.Npad * 128u);
-            for (int c = 0; c < p.nchunks; ++c)
-                tma_load_3d(base + sm.w + (uint32_t)c * p.w_tile_bytes, &tmW, w_full, p.c_slot[c] * 64, 0, 0);
-            asm volatile("griddepcontrol.wait;" ::: "memory");
-            // ONE operand stage per tile: all K chunks of a tile share a stage and a barrier pair. A chunk is only a few long MMAs
-            // here (N' up to 240), and every stage hand-off costs the tensor pipe a few hundred idle cycles (DESIGN.md): per-chunk
-            // stages left the pipe idle two thirds of the time (profiles/r02_tn_roles.txt).
-            uint32_t it = 0;
-            for (int tile = first_tile; tile < total_tiles; tile += gridDim.x, ++it) {
-                int b0, l0;
-                tile_coords(tile, b0, l0);
-                const uint32_t sa = it % (uint32_t)p.na, pa = (it / (uint32_t)p.na) & 1u;
-                mbar_wait(a_empty + 8 * sa, pa ^ 1);
-                if (p.ntma == 0 || (DBG & 16)) { mbar_arrive(a_full + 8 * sa); continue; }
-                mbar_expect_tx(a_full + 8 * sa, (uint32_t)p.ntma * (uint32_t)nblk * 4096u);
-                for (int c = 0; c < p.nchunks; ++c) {
-                    if (p.c_up[c]) continue;
-                    const uint32_t dst = base + sm.a + sa * p.a_stage_bytes + (uint32_t)c * p.a_sub_bytes;
-                    const int lc = l0 - p.pad + p.c_row[c];
-                    for (int k = 0; k < nblk; ++k)
-                        tma_load_3d(dst + (uint32_t)k * 4096u, &tmA, a_full + 8 * sa, p.c_ch[c] * 64, lc + 28 * k, b0);
-                }
-            }
-        }
-    } else if (warp == kMmaWarp) {
-        if (elect_one()) {
-            const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.Npad >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            mbar_wait(w_full, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            int it = 0;
-            for (int tile = first_tile; tile < total_tiles; tile += gridDim.x, ++it) {
-                const int buf = it & 1;
-                const uint32_t sa = (uint32_t)it % (uint32_t)p.na, pa = ((uint32_t)it / (uint32_t)p.na) & 1u;
-                mbar_wait(acc_empty + 8 * buf, (((uint32_t)it >> 1) & 1u) ^ 1u);
-                mbar_wait(a_full + 8 * sa, pa);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t acc_col = tmem_base + (uint32_t)(buf * p.MT * p.Nstride);
-                const uint32_t a_stage = (((base + sm.a + sa * p.a_stage_bytes) >> 4) & 0x3FFFu) | (1u << 16);
-#pragma unroll 1
-                for (int c = 0; c < p.nchunks; ++c) {
-                    const uint32_t a_lo = a_stage + (uint32_t)c * (p.a_sub_bytes >> 4);
-                    const uint32_t b_lo = (((base + sm.w + (uint32_t)c * p.w_tile_bytes) >> 4) & 0x3FFFu) | (1u << 16);
-                    const int nk = p.c_nk[c];
-#pragma unroll 1
-                    for (int mt = 0; mt < ((DBG & 8) ? 0 : p.MT); ++mt) {
-                        const uint32_t d = acc_col + (uint32_t)(mt * p.Nstride);
-                        const uint32_t am = a_lo + (uint32_t)mt * 1024u;               // next 128 rows: 16 KB = 1024 sixteen-byte units
-                        umma_bf16_lohi(d, am, b_lo, hi, idesc, c ? 1u : 0u);
-                        if (nk > 1) umma_bf16_lohi(d, am + 2, b_lo + 2, hi, idesc, 1u);
-                        if (nk > 2) umma_bf16_lohi(d, am + 4, b_lo + 4, hi, idesc, 1u);
-                        if (nk > 3) umma_bf16_lohi(d, am + 6, b_lo + 6, hi, idesc, 1u);
-                    }
-                }
-                umma_commit(a_empty + 8 * sa);
-                umma_commit(acc_full + 8 * buf);
-            }
-        }
-    } else if (warp < EW) {
-        // ======================= epilogue: shifted tap sum + BatchNorm + LeakyReLU (+ fused head) =======================
-        const int q = warp & 3, half = warp >> 2;
-        const float2 *ss = reinterpret_cast<const float2 *>(base_ptr + sm.ss);
-        const float *hw = reinterpret_cast<const float *>(base_ptr + sm.ss) + 2 * p.Cout;
-        const int ncc = p.Cout >> 3;                              // 8-column chunks of the output
-        int it = 0;
-        for (int tile = first_tile; tile < total_tiles; tile += gridDim.x, ++it) {
-            int b0, l0;
-            tile_coords(tile, b0, l0);
-            const int buf = it & 1;
-            // fused head: the raw-input samples of this thread's rows, fetched before the accumulators are waited for
-            float xin[4] = {0.f, 0.f, 0.f, 0.f};
-            if (p.head) {
-#pragma unroll
-                for (int mt = 0; mt < 4; ++mt) {
-                    const int l = l0 + 28 * (4 * mt + q) + lane;
-                    if (mt < p.MT && (mt & 1) == half && lane < 28 && l < p.L) xin[mt] = __ldg(p.x + (size_t)b0 * p.T + l);
-                }
-            }
-            mbar_wait(acc_full + 8 * buf, ((uint32_t)it >> 1) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int mt = 0; mt < p.MT; ++mt) {
-                // the two warps of a quadrant split the work: by sub-tile when there are several, else by column chunk
-                if (p.MT > 1 && (mt & 1) != half) continue;
-                const int l = l0 + 28 * (4 * mt + q) + lane;
-                const bool valid = lane < 28 && l < p.L;
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((buf * p.MT + mt) * p.Nstride);
-                float hacc = p.head ? hw[p.Cout + 1] : 0.f;
-#pragma unroll 1
-                for (int cc = (p.MT > 1 ? 0 : half); cc < ncc; cc += (p.MT > 1 ? 1 : 2)) {
-                    uint32_t v0[8], v1[8], v2[8], v3[8], v4[8];
-                    const uint32_t col = taddr + (uint32_t)(8 * cc);
-                    if (DBG & 1) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) { v0[j] = col + j; v1[j] = col ^ j; v2[j] = col * j; v3[j] = col - j; v4[j] = j; }
-                    } else {
-                    tmem_ld8_nowait(col, v0);
-                    tmem_ld8_nowait(col + (uint32_t)p.Cp, v1);
-                    tmem_ld8_nowait(col + (uint32_t)(2 * p.Cp), v2);
-                    tmem_ld8_nowait(col + (uint32_t)(3 * p.Cp), v3);
-                    tmem_ld8_nowait(col + (uint32_t)(4 * p.Cp), v4);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    }
-                    float f[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        // out[row] = D'[row,0] + D'[row+1,1] + ... + D'[row+4,4]; lanes 28..31 end up incomplete and are not stored
-                        float a = __uint_as_float(v4[j]);
-                        if (DBG & 2) {
-                            a = a + __uint_as_float(v3[j]) + __uint_as_float(v2[j]) + __uint_as_float(v1[j]) + __uint_as_float(v0[j]);
-                        } else {
-                        a = __shfl_down_sync(0xffffffffu, a, 1) + __uint_as_float(v3[j]);
-                        a = __shfl_down_sync(0xffffffffu, a, 1) + __uint_as_float(v2[j]);
-                        a = __shfl_down_sync(0xffffffffu, a, 1) + __uint_as_float(v1[j]);
-                        a = __shfl_down_sync(0xffffffffu, a, 1) + __uint_as_float(v0[j]);
-                        }
-                        const float2 s2 = ss[8 * cc + j];
-                        f[j] = lrelu(fmaf(a, s2.x, s2.y));
-                    }
-                    if (p.out != nullptr && valid && !(DBG & 4))
-                        *reinterpret_cast<uint4 *>(p.out + ((size_t)b0 * p.L + l) * p.Cout + 8 * cc) =
-                            make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-                    if (p.head) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) hacc = fmaf(hw[8 * cc + j], f[j], hacc);
-                    }
-                }
-                if (p.head && valid && !(DBG & 4)) {
-                    // cat([o, input], 1) -> Conv1d(C+1 -> 1, k=1) -> Tanh   (model/unet_basic.py:98-99)
-                    hacc = fmaf(hw[p.Cout], mt == 0 ? xin[0] : (mt == 1 ? xin[1] : (mt == 2 ? xin[2] : xin[3])), hacc);
-                    p.y[(size_t)b0 * p.T + l] = tanh_fast(hacc);
-                }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty + 8 * buf);
-        }
-    } else if (UPCAT) {
-        // ======================= upsample producers =======================
-        // As in conv_tc_kernel (16 output rows x one 16-byte channel vector per thread, packed-bf16 interpolation straight into
-        // the swizzled operand), with the operand rows mapped to positions block by block (row 32 k + i <-> l0 - PAD + 28 k + i)
-        // and the producer warps split into groups that work on different TILES at the same time: a tile has fewer items
-        // than there are producer threads, and an item's latency (~1.5 k cycles + its loads) is longer than a tile's MMAs.
-        const int pw = warp - kFirstProducer;
-        const int grp = pw / p.wpg;
-        if (grp < p.npg && p.nup_items > 0) {
-            const int pt = (pw - grp * p.wpg) * 32 + lane;
-            const int nthreads = p.wpg * 32;
-            // items of a tile: for every upsampled chunk (16-row run, 16-byte channel vector); a group owns every npg-th tile
-            uint32_t it = 0;
-            for (int tile = first_tile; tile < total_tiles; tile += gridDim.x, ++it) {
-                int b0, l0;
-                tile_coords(tile, b0, l0);
-                // Every group follows EVERY tile's stage release in order, also of the tiles it does not write: an mbarrier wait
-                // only tells the current phase from the previous one, so a waiter must never get two uses of a stage ahead of
-                // (or behind) the barrier it polls.
-                const uint32_t sa = it % (uint32_t)p.na, pa = (it / (uint32_t)p.na) & 1u;
-                const bool mine = (it % (uint32_t)p.npg) == (uint32_t)grp;
-                if (!mine) { mbar_wait(a_empty + 8 * sa, pa ^ 1); continue; }
-                if (DBG & 32) {
-                    mbar_wait(a_empty + 8 * sa, pa ^ 1);
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(a_full + 8 * sa);
-                    continue;
-                }
-                uint4 xr[10];
-                // item -> (chunk c, run, vec): the upsampled chunks are laid out one after the other in the item index
-                auto locate = [&](int item, int &c, int &run, int &vec) {
-                    c = 0;
-                    for (;; ++c) {
-                        if (!p.c_up[c]) continue;
-                        const int n = 8 * p.MT * 2 * (int)p.c_nk[c];
-                        if (item < n) break;
-                        item -= n;
-                    }
-                    const int nvec = 2 * (int)p.c_nk[c];
-                    run = item / nvec; vec = item - run * nvec;
-                };
-                auto fetch = [&](int c, int run, int vec) {
-                    const int ch = p.c_ch[c] * 64 + vec * 8;
-                    const int lstart = l0 - p.pad + 28 * (run >> 1) + 16 * (run & 1);      // even
-                    const int ms = lstart >> 1;
-                    const bool chok = ch < p.Cin0;
-                    const __nv_bfloat16 *pb = p.prev + (size_t)b0 * p.Lin * p.Cin0 + ch;
-#pragma unroll
-                    for (int qq = 0; qq < 10; ++qq) {
-                        int m = ms - 1 + qq;
-                        m = m < 0 ? 0 : (m > p.Lin - 1 ? p.Lin - 1 : m);
-                        xr[qq] = chok ? __ldg(reinterpret_cast<const uint4 *>(pb + (size_t)m * p.Cin0)) : make_uint4(0u, 0u, 0u, 0u);
-                    }
-                };
-                int c = 0, run = 0, vec = 0;
-                if (pt < p.nup_items) { locate(pt, c, run, vec); fetch(c, run, vec); }     // issued before the wait: DRAM latency overlaps it
-                mbar_wait(a_empty + 8 * sa, pa ^ 1);
-                const uint32_t stage = base + sm.a + sa * p.a_stage_bytes;
-#pragma unroll 1
-                for (int item = pt; item < p.nup_items; item += nthreads) {
-                    if (item != pt) { locate(item, c, run, vec); fetch(c, run, vec); }
-                    const int ch = p.c_ch[c] * 64 + vec * 8;
-                    const int lstart = l0 - p.pad + 28 * (run >> 1) + 16 * (run & 1);
-                    const int ms = lstart >> 1;
-                    const bool chok = ch < p.Cin0;
-                    const float lf0 = (float)lstart, mf0 = (float)(ms - 1);
-                    const uint32_t drow = stage + (uint32_t)c * p.a_sub_bytes + (uint32_t)(16 * run) * 128u;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int l = lstart + j;
-                        const int qa = (j >> 1) + (j & 1);
-                        const float lam1 = fmaf(p.up_scale, lf0 + (float)j, -(mf0 + (float)qa));
-                        const __nv_bfloat162 lam = __float2bfloat162_rn(lam1);
-                        const __nv_bfloat162 *a2 = reinterpret_cast<const __nv_bfloat162 *>(&xr[qa]);
-                        const __nv_bfloat162 *b2 = reinterpret_cast<const __nv_bfloat162 *>(&xr[qa + 1]);
-                        __nv_bfloat162 r2[4];
-#pragma unroll
-                        for (int q4 = 0; q4 < 4; ++q4) r2[q4] = __hfma2(lam, __hsub2(b2[q4], a2[q4]), a2[q4]);
-                        uint4 o = *reinterpret_cast<const uint4 *>(r2);
-                        const uint32_t keep = (chok && (unsigned)l < (unsigned)p.L) ? 0xffffffffu : 0u;
-                        o.x &= keep; o.y &= keep; o.z &= keep; o.w &= keep;
-                        st_shared_v4_if(drow + (uint32_t)(j * 128 + ((vec ^ (j & 7)) << 4)), o, true);
-                    }
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(a_full + 8 * sa);
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == kMmaWarp) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols));
-}
-
-// TN weights: [Npad rows = (t', co) at t' * Cp + co][nslots * 64] bf16. Decoder (ngroups == 1): K slots as in pack_tc_kernel
-// ([upsampled chunks | skip chunks], 64 channels each), tap = t'. Encoder: slot g = tap group g (taps 5 g + t'), channel < Cin.
-__global__ void pack_tn_kernel(const float *__restrict__ w, __nv_bfloat16 *__restrict__ wp, int Cout, int Cin0, int Cin1, int K,
-                               int Cp, int Npad, int nslots, int ngroups)
-{
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long n = (long long)Npad * nslots * 64;
-    if (i >= n) return;
-    const int ks = (int)(i % (nslots * 64));
-    const int row = (int)(i / (nslots * 64));
-    const int tp = row / Cp, co = row - tp * Cp;
-    float v = 0.f;
-    if (tp < 5 && co < Cout) {
-        int ci = -1, tap = tp;
-        if (ngroups == 1) {
-            const int seg1_base = (Cin0 + 63) / 64 * 64;
-            if (ks < seg1_base) { if (ks < Cin0) ci = ks; }
-            else if (ks - seg1_base < Cin1) ci = Cin0 + (ks - seg1_base);
-        } else {
-            const int g = ks / 64, c = ks - g * 64;
-            tap = 5 * g + tp;
-            if (c < Cin0 && g < ngroups) ci = c;
-        }
-        if (ci >= 0 && tap < K) v = w[((size_t)co * (Cin0 + Cin1) + ci) * K + tap];
-    }
-    wp[i] = __float2bfloat16(v);
 }
 
 // -------------------------------------------------------------------------------------------------
 // bottom of the U (frames of at most 16 samples): the block as ONE dense GEMM over frames
 // -------------------------------------------------------------------------------------------------
-// With L <= 16 the implicit GEMM over positions wastes 60-80 % of its MMA rows on per-frame halos and cannot fill the SMs.
+// With L <= 16 the implicit GEMM over positions wastes most of its MMA rows on per-frame halos and cannot fill the SMs.
 // Here the frames are the GEMM rows: the channels-last activations ARE the matrix [B][L*C],
 //     Y[b][(l, co)] = sum_(l', ci) X[b][(l', ci)] * W'[(l, co)][(l', ci)],
 // with Toeplitz-expanded weights W'[(l,co)][(l',ci)] = w[co][ci][l'-l+pad] (zero outside the taps; built once per weight
-// update by expand_*_kernel). An encoder's decimation is the tensor map's row stride; a decoder's linear interpolation is
-// folded into the expanded weights of its upsampled input (W * U, in fp32, then bf16), so both of its sources are plain TMA
-// operands and there are no producer warps. One CTA = 128 frames x Nh output columns; K runs over 64-channel chunks of the
-// input positions that reach the CTA's output positions (the band), several chunks per pipeline stage.
+// update by expand_gemm_weights_kernel). An encoder's decimation is the tensor map's row stride; a decoder's linear
+// interpolation is folded into the expanded weights of its upsampled input (W * U, in fp32, then bf16), so both of its sources
+// are plain TMA operands and there are no producer warps. One CTA = 128 frames x Nh output columns (two consumer warpgroups of
+// 64 frames each, accumulators in registers); K runs over 64-channel chunks of the input positions that reach the CTA's output
+// positions (the band), several chunks per pipeline stage.
 struct GemmParams {
-    int B, N, Nh;                  // rows (frames), output columns (= L * Cout), columns per CTA
+    int B, N, Nh;                  // rows (frames), output columns (= L * Cout), columns per CTA (<= kAccColsLarge)
     int cout;                      // channels per output position (the folded BatchNorm vector repeats with this period)
     int L;                         // output positions
     // two sources: chunk list = [source 0 positions x 64-channel chunks | source 1 positions x chunks]; weight K slot = global index
@@ -1674,42 +1089,34 @@ struct GemmParams {
     int reach_lo[2], reach_hi[2];  // input positions [l_lo + reach_lo, l_hi + reach_hi] reach output positions [l_lo, l_hi]; for a
     int halve[2];                  // half-resolution source (decoder: previous block) the output range is halved first
     int nstages, cps;              // ring depth, K chunks per stage
-    uint32_t a_bytes, w_bytes, tmem_cols;
+    uint32_t a_bytes, w_bytes;
     const float2 *ss;              // [cout] folded BatchNorm (scale, shift)
     __nv_bfloat16 *out;            // [B][N]
 };
+constexpr int kGemmThreads = 32 * (kEpiWarpsLarge + 1);   // two consumer warpgroups + the TMA warp
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tmW,
                const GemmParams p)
 {
+    constexpr int NWG = kEpiWarpsLarge / 4;
+    constexpr int NB = kAccColsLarge / 16;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    // a stage holds `cps` consecutive K chunks: [A: cps x 16 KB (128 frames x 64 channels each) | W: cps x w_bytes]. Every stage
-    // hand-off idles the tensor pipe for a few hundred cycles and a chunk is only 4 short MMAs: fat stages amortise it.
+    // a stage holds `cps` consecutive K chunks: [A: cps x 16 KB (128 frames x 64 channels each) | W: cps x w_bytes]
     const uint32_t stage_bytes = (uint32_t)p.cps * (16384u + p.w_bytes);
-    const uint32_t bars = base + (uint32_t)p.nstages * stage_bytes;                 // full[8] empty[8] acc | tmem slot
-    const uint32_t full = bars, empty = bars + 64, acc_full = bars + 128, tmem_slot = bars + 136;
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(base_ptr + (size_t)p.nstages * stage_bytes + 136);
+    const uint32_t bars = base + (uint32_t)p.nstages * stage_bytes;                 // full[8] empty[8]
+    const uint32_t full = bars, empty = bars + 64;
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = blockIdx.x * p.Nh, b0 = blockIdx.y * 128;
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm0)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
-        for (int s = 0; s < 8; ++s) { mbar_init(full + 8 * s, 1); mbar_init(empty + 8 * s, 1); }
-        mbar_init(acc_full, 1);
+        for (int s = 0; s < 8; ++s) { mbar_init(full + 8 * s, 1); mbar_init(empty + 8 * s, NWG); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 5) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(p.tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot_ptr;
     asm volatile("griddepcontrol.wait;" ::: "memory");
 
     // the band: input positions of each source that reach this CTA's output positions
@@ -1725,7 +1132,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     }
     const int nst = (nch + p.cps - 1) / p.cps;                   // stages of this CTA's K loop
     const int n_this = min(p.Nh, p.N - n0);
-    if (warp == 4) {
+    if (warp == kEpiWarpsLarge) {
+        // ======================= TMA producer =======================
         if (lane == 0) {
             for (int it = 0; it < nst; ++it) {
                 const uint32_t st = (uint32_t)it % (uint32_t)p.nstages, ph = ((uint32_t)it / (uint32_t)p.nstages) & 1u;
@@ -1743,56 +1151,53 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 5) {
-        if (elect_one()) {
-            const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.Nh >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            for (int it = 0; it < nst; ++it) {
-                const uint32_t st = (uint32_t)it % (uint32_t)p.nstages, ph = ((uint32_t)it / (uint32_t)p.nstages) & 1u;
-                const int kn = min(p.cps, nch - it * p.cps);
-                mbar_wait(full + 8 * st, ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a0 = (((base + st * stage_bytes) >> 4) & 0x3FFFu) | (1u << 16);
-                const uint32_t w0 = (((base + st * stage_bytes + (uint32_t)p.cps * 16384u) >> 4) & 0x3FFFu) | (1u << 16);
-#pragma unroll 1
-                for (int j = 0; j < kn; ++j) {
-                    const uint32_t a_lo = a0 + (uint32_t)j * 1024u, b_lo = w0 + (uint32_t)j * (p.w_bytes >> 4);
-                    umma_bf16_lohi(tmem_base, a_lo, b_lo, hi, idesc, (it | j) ? 1u : 0u);
-                    umma_bf16_lohi(tmem_base, a_lo + 2, b_lo + 2, hi, idesc, 1u);
-                    umma_bf16_lohi(tmem_base, a_lo + 4, b_lo + 4, hi, idesc, 1u);
-                    umma_bf16_lohi(tmem_base, a_lo + 6, b_lo + 6, hi, idesc, 1u);
-                }
-                umma_commit(empty + 8 * st);
-            }
-            umma_commit(acc_full);
-        }
     } else {
-        // epilogue: warp q owns TMEM lanes (= frames) 32 q .. 32 q + 31
-        const int q = warp;
-        mbar_wait(acc_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int b = b0 + q * 32 + lane;
-#pragma unroll 1
-        for (int c16 = 0; c16 < n_this; c16 += 16) {
-            uint32_t v[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c16, v);
-            uint32_t o[8];
+        // ======================= consumer warpgroups: wgmma over 64 frames each + epilogue =======================
+        const int wg = warp >> 2, wq = warp & 3;
+        const int nblk = n_this >> 4;
+        const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 30);
+        float acc[NB][8];
 #pragma unroll
-            for (int j = 0; j < 16; j += 2) {
-                const int n = n0 + c16 + j;
-                const float2 s0 = __ldg(p.ss + n % p.cout), s1 = __ldg(p.ss + (n + 1) % p.cout);
-                o[j >> 1] = pack_bf16(lrelu(fmaf(__uint_as_float(v[j]), s0.x, s0.y)), lrelu(fmaf(__uint_as_float(v[j + 1]), s1.x, s1.y)));
+        for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[nb][j] = 0.f;
+        for (int it = 0; it < nst; ++it) {
+            const uint32_t st = (uint32_t)it % (uint32_t)p.nstages, ph = ((uint32_t)it / (uint32_t)p.nstages) & 1u;
+            const int kn = min(p.cps, nch - it * p.cps);
+            mbar_wait(full + 8 * st, ph);
+            const uint32_t a0 = (((base + st * stage_bytes) >> 4) & 0x3FFFu) | (1u << 16);
+            const uint32_t w0 = (((base + st * stage_bytes + (uint32_t)p.cps * 16384u) >> 4) & 0x3FFFu) | (1u << 16);
+            wgmma_fence();
+#pragma unroll 1
+            for (int j = 0; j < kn; ++j) {
+                const uint32_t a_lo = a0 + (uint32_t)j * 1024u + (uint32_t)wg * 512u, b_lo = w0 + (uint32_t)j * (p.w_bytes >> 4);
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+#pragma unroll
+                    for (int nb = 0; nb < NB; ++nb)
+                        if (nb < nblk) wgmma_n16(acc[nb], a_lo + 2 * k, b_lo + (uint32_t)(nb * 128 + 2 * k), hi);
             }
-            if (b < p.B) {
-                uint4 *dst = reinterpret_cast<uint4 *>(p.out + (size_t)b * p.N + n0 + c16);
-                dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
-                dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
+            wgmma_commit();
+            wgmma_wait0();
+            if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * st);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int b = b0 + wg * 64 + 16 * wq + (lane >> 2) + 8 * h;
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) {
+                if (nb >= nblk) break;
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = n0 + nb * 16 + 8 * e + 2 * (lane & 3);
+                    const float2 s0 = __ldg(p.ss + n % p.cout), s1 = __ldg(p.ss + (n + 1) % p.cout);
+                    const uint32_t o = pack_bf16(lrelu(fmaf(acc[nb][4 * e + 2 * h], s0.x, s0.y)),
+                                                 lrelu(fmaf(acc[nb][4 * e + 2 * h + 1], s1.x, s1.y)));
+                    if (b < p.B) *reinterpret_cast<uint32_t *>(p.out + (size_t)b * p.N + n) = o;
+                }
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 5) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols));
 }
 
 // Toeplitz expansion of a block's weights for gemm_tc_kernel: wx[n = l * Cout + co][k], K slots of 64 channels:
@@ -2223,9 +1628,6 @@ struct TcLevel {
     size_t wx_elems = 0;
     __nv_bfloat16 *wp_sp = nullptr;    // split-precision packing [K][Npad][sp_chunks * 64] (sp_chunk_order lists the K-loop positions)
     int sp_chunks = 0;
-    // taps-in-N variant (conv_tn_kernel): eligible blocks keep a second packed copy [tn_npad][tn_slots * 64]
-    int tn_cp = 0, tn_npad = 0, tn_slots = 0, tn_groups = 0;      // 0 = not eligible
-    __nv_bfloat16 *wp_tn = nullptr;
     const float *w_src = nullptr;      // enc0 only: fp32 weights (w_own, a library-owned copy) / scale / shift (the context's folded copies)
     float *w_own = nullptr;            // enc0 only: [Cout][1][K] fp32 copy made by tc_set_weights (the caller's tensor is not read afterwards)
     const float *scale = nullptr, *shift = nullptr;
@@ -2237,8 +1639,6 @@ struct TcPlanLevel {
     TcParams p;
     GemmParams gp;                     // is_gemm: the block runs gemm_tc_kernel (tmA / tmO = its two sources, tmW = expanded weights)
     bool is_gemm = false;
-    TnParams tn;                       // is_tn: the block runs conv_tn_kernel (tmA / tmW are its maps, p is unused)
-    bool is_tn = false;
     CUtensorMap tmA, tmW, tmO;
     dim3 grid;
     int threads;
@@ -2247,14 +1647,14 @@ struct TcPlanLevel {
     bool upcat;
     bool small;                        // two-CTAs-per-SM kernel flavour
     int kind = 0;                      // reported by wunet_debug_plan in the 'small' field: 2 = dense GEMM over frames (gemm_tc_kernel)
-    int pair = 0;                      // row-pair mode: 1 = encoder block (conv_tc_kernel<9, false, ...>), 2 = last decoder block (<3, true, ..., PR = 1>);
+    int pair = 0;                      // row-pair mode: 1 = encoder block (conv_tc_kernel<9, false, ...>), 
                                        // 3 = block 0 over groups of 8 samples (<3, false, ...>)
 };
 
 // Per-block tiling overrides for tuning sweeps: WUNET_TC_OVR="<block>:key=val,key=val;<block>:..." with keys
-// mt, ns (column splits), na, nacc, tg, res (0/1), small (0/1), bulk (0/1), packed (1: pack L=128 frames). Unset keys keep
+// mt, ns (column splits), na, nacc, tg, res (0/1), small (0/1), packed (1: pack L=128 frames). Unset keys keep
 // the heuristic's choice.
-struct TcOverride { int mt = 0, ns = 0, na = 0, nacc = 0, tg = 0, nb = 0, res = -1, small = -1, bulk = -1, packed = -1; bool any = false; };
+struct TcOverride { int mt = 0, ns = 0, na = 0, nacc = 0, tg = 0, nb = 0, res = -1, small = -1, packed = -1; bool any = false; };
 static void parse_kv(const std::string &seg, TcOverride &ov)
 {
     size_t q = 0;
@@ -2269,7 +1669,7 @@ static void parse_kv(const std::string &seg, TcOverride &ov)
         const int v = atoi(kv.c_str() + eq + 1);
         if (k == "mt") ov.mt = v; else if (k == "ns") ov.ns = v; else if (k == "na") ov.na = v;
         else if (k == "nacc") ov.nacc = v; else if (k == "tg") ov.tg = v; else if (k == "res") ov.res = v;
-        else if (k == "small") ov.small = v; else if (k == "bulk") ov.bulk = v; else if (k == "packed") ov.packed = v;
+        else if (k == "small") ov.small = v; else if (k == "packed") ov.packed = v;
         else if (k == "nb") ov.nb = v;
         ov.any = true;
     }
@@ -2290,19 +1690,6 @@ static TcOverride parse_override(const std::string &env, int block)
     return ov;
 }
 
-// Tilings found by tools/sweep_levels.py on a B200 for the reference's default architecture (12 levels x 24 channels,
-// 16384-sample frames, batch 256) where they beat the generic rules of build_plan by more than 3 %. Keyed on the block's
-// shape, used for batches >= 128 frames (the tile-count regime they were measured in); anything else takes the rules.
-struct TunedTiling { int L, cin0, cin1, cout, k; const char *kv; };
-static const TunedTiling kTuned[] = {
-    {64, 192, 0, 216, 15, "mt=3,ns=2"},               // enc8:  34.3 us vs 38.6
-    {32, 216, 0, 240, 15, "mt=1,ns=3,small=1"},       // enc9:  25.9 us vs 29.2
-    {64, 240, 216, 216, 5, "mt=1,ns=1,small=1"},      // dec3:  37.3 us vs 38.9
-    {128, 216, 192, 192, 5, "mt=1,small=1"},          // dec4:  34.7 us vs 36.4
-    {512, 168, 144, 144, 5, "mt=1,small=1"},          // dec6:  73.8 us vs 77.9
-    {16384, 48, 24, 24, 5, "mt=2,small=1"},           // dec11 + head: 245 us vs 262
-};
-
 struct TcPlan {
     std::vector<TcPlanLevel> lv;       // index 1..2n (0 = enc0 handled separately)
     std::vector<size_t> off;           // workspace offsets of the 2n+1 block outputs (+ the even-row copy of block 0)
@@ -2316,24 +1703,18 @@ struct TcState {
     const float *out_w = nullptr, *out_b = nullptr;
     EncodeTiledFn encode = nullptr;
     bool store_last = false;           // WUNET_TC_STORE_LAST=1: also materialise the last decoder block (tests)
-    bool headk = false;                // WUNET_TC_HEADK=1: head-only instantiation for the last block (bit-identical; slower at the
-                                       // tiling its shared-memory ring allows, DESIGN.md)
-    int head_mt = 1;                   // its M sub-tiles per CTA (WUNET_TC_HEADMT)
     int enc_l2promo = 256;             // L2 promotion of the encoders' decimated input views (WUNET_TC_L2PROMO = 0 / 64 / 128 / 256)
     bool attr_set = false;
     bool pdl = false;                  // programmatic dependent launch between the blocks (WUNET_TC_PDL=1); measured slower, off
     bool merge = true;                 // merged tail chunks (WUNET_TC_MERGE=0 switches them off for A/B measurements)
     bool pf_late = false;              // WUNET_TC_PFLATE=1: see TcParams::pf_late
     bool gemm = true;                  // dense GEMM over frames for blocks of at most 16 samples (WUNET_TC_GEMM=0 switches it off)
-    bool tn = false;                   // taps-in-N kernel for the shallow blocks: correct but not yet faster than conv_tc_kernel on a B200
-                                       // (profiles/r02_tn_*.txt), so opt-in: WUNET_TC_TN=1
     // row-pair mode (WUNET_TC_PAIR bit 0: first tensor-core encoder block, bit 1: last decoder block + head): virtual blocks with
     // doubled channel counts and Toeplitz-expanded weights (pair_weight), planned on frames of half the length
-    int pair_mask = 1;                 // default: block 1 in row-pair mode (127 -> 97 us at batch 256; +8 us in enc0 for the even-row copy),
-                                       // the last block not (its pair form is slower: 241 -> 300 us, profiles/r02_row_pair_ab.txt)
+    int pair_mask = 1;                 // default: block 1 in row-pair mode (enc0 also writes a dense copy of its even rows)
     int enc0_v = 0;                    // WUNET_TC_ENC0V: 2 = persistent form of the CUDA-core enc0 kernel (bit-identical), 1 = one tile per block,
-                                       // 0 (default) = persistent for the split-precision path (two blocks per SM there: 64 -> 53 us at batch 64), one
-                                       // tile per block for bf16 (four blocks per SM overlap their phases already: 115 vs 117 us, tools/enc0v_check.py)
+                                       // 0 (default) = persistent for the split-precision path (two blocks per SM there), one
+                                       // tile per block for bf16 (four blocks per SM overlap their phases already)
     bool enc0_tc = false;              // WUNET_TC_ENC0=1: block 0 on the tensor cores in its group-of-8 form (group8_weight); bf16 mode only
     bool enc0_ok = false;
     TcLevel g8_lv;                     // its virtual block: 8 input channels, 8 C columns, 3 taps
@@ -2387,7 +1768,7 @@ size_t tc_workspace_bytes(int n, int ci, int B, int T, int mode)
 
 // K segments and padded sizes of every block: encoders have one input segment, decoder block i concatenates the previous
 // block's (upsampled) output with the skip of encoder 2n - i (model/unet_basic.py:93-95)
-static void derive_levels(std::vector<TcLevel> &levels, const TcBlockSrc *blocks, int nblocks, int n, bool merge = true, bool tn = true)
+static void derive_levels(std::vector<TcLevel> &levels, const TcBlockSrc *blocks, int nblocks, int n, bool merge = true)
 {
     for (int i = 0; i < nblocks; ++i) {
         TcLevel &lv = levels[i];
@@ -2398,15 +1779,6 @@ static void derive_levels(std::vector<TcLevel> &levels, const TcBlockSrc *blocks
         lv.Ktot = round_up(lv.cin0, 64) + (lv.cin1 ? round_up(lv.cin1, 64) : 0);
         lv.w_src = blocks[i].w; lv.scale = blocks[i].scale; lv.shift = blocks[i].shift;
         lv.mg_s = lv.mg_u = 0;
-        // taps-in-N: 5 taps x Cout columns must fit one MMA (N <= 256) and pay off (N = Cout < 64: operand-read-bound MMAs)
-        lv.tn_cp = lv.tn_npad = lv.tn_slots = lv.tn_groups = 0;
-        if (tn && i >= 1 && lv.cout % 8 == 0 && lv.cout <= 48 && lv.k % 5 == 0) {
-            const int groups = lv.k / 5;
-            const int slots = (i > n) ? (lv.cin0 + 63) / 64 + (lv.cin1 + 63) / 64 : groups * ((lv.cin0 + 63) / 64);
-            if (((i > n && groups == 1) || (i <= n && lv.cin0 <= 64)) && slots <= 8) {
-                lv.tn_cp = lv.cout; lv.tn_npad = round_up(5 * lv.cout, 16); lv.tn_slots = slots; lv.tn_groups = groups;
-            }
-        }
         const int u = lv.cin0 % 64, sk = lv.cin1 % 64;
         if (merge && i > n && u > 0 && sk > 0 && u + sk <= 64 && u % 8 == 0 && sk % 8 == 0) {
             lv.mg_s = sk; lv.mg_u = u;
@@ -2436,11 +1808,8 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         const char *pe = getenv("WUNET_TC_PDL");
         st->pdl = pe && pe[0] == '1';
         if (const char *xe = getenv("WUNET_TC_MERGE")) st->merge = xe[0] != '0';
-        if (const char *xe = getenv("WUNET_TC_TN")) st->tn = xe[0] == '1';
-        if (const char *xe = getenv("WUNET_TC_GEMM")) st->gemm = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_PFLATE")) st->pf_late = xe[0] == '1';
-        if (const char *xe = getenv("WUNET_TC_HEADK")) st->headk = xe[0] == '1';
-        if (const char *xe = getenv("WUNET_TC_HEADMT")) st->head_mt = std::max(1, std::min(4, atoi(xe)));
+        if (const char *xe = getenv("WUNET_TC_GEMM")) st->gemm = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_L2PROMO")) st->enc_l2promo = atoi(xe);
         if (const char *xe = getenv("WUNET_TC_PAIR")) st->pair_mask = atoi(xe) & 3;
         if (const char *xe = getenv("WUNET_TC_ENC0")) st->enc0_tc = xe[0] == '1';
@@ -2456,7 +1825,7 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
     }
     st->out_w = out_w; st->out_b = out_b;
     st->plan_ws = nullptr;                               // weights moved: rebuild maps lazily
-    derive_levels(st->levels, blocks, nblocks, n, st->merge, st->tn);
+    derive_levels(st->levels, blocks, nblocks, n, st->merge);
     if (ci % 8 != 0 || ci > 32) return 0;                // tensor-core path unsupported for this plan; forward reports it
     {
         // enc0 runs on CUDA cores from fp32 weights: keep a library-owned copy (include/wunet_b200.h: the caller's tensors are
@@ -2495,13 +1864,6 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
                                                                                   lv.Npad, tab);
             if (cudaGetLastError() != cudaSuccess) return tc_fail("pack_tc_split_kernel launch failed");
         }
-        if (lv.tn_slots) {
-            const size_t nt = (size_t)lv.tn_npad * lv.tn_slots * 64;
-            if (!lv.wp_tn && cudaMalloc(&lv.wp_tn, nt * sizeof(__nv_bfloat16)) != cudaSuccess) return tc_fail("cudaMalloc(wp_tn) failed");
-            pack_tn_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, stream>>>(blocks[i].w, lv.wp_tn, lv.cout, lv.cin0, lv.cin1, lv.k, lv.tn_cp,
-                                                                            lv.tn_npad, lv.tn_slots, lv.tn_groups);
-            if (cudaGetLastError() != cudaSuccess) return tc_fail("pack_tn_kernel launch failed");
-        }
         if (lv.mg_s) {
             const size_t nm = (size_t)lv.k * lv.Npad * 64;
             pack_tc_merged_kernel<<<(unsigned)((nm + 255) / 256), 256, 0, stream>>>(blocks[i].w, lv.wp, lv.cout, lv.cin0, lv.cin1, lv.k,
@@ -2517,7 +1879,6 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         pv.cin0 = 8; pv.cin1 = 0; pv.cout = 8 * rl.cout; pv.k = 3;
         pv.Npad = round_up(pv.cout, 16); pv.Ktot = 64;
         pv.mg_s = pv.mg_u = 0;
-        pv.tn_cp = pv.tn_npad = pv.tn_slots = pv.tn_groups = 0;
         const size_t nv = (size_t)pv.cout * 8 * 3, nel = (size_t)3 * pv.Npad * pv.Ktot;
         if (!st->g8_w) {
             if (cudaMalloc(&st->g8_w, nv * sizeof(float)) != cudaSuccess || cudaMalloc(&st->g8_scale, pv.cout * sizeof(float)) != cudaSuccess ||
@@ -2534,7 +1895,7 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         st->enc0_ok = true;
     }
     // row-pair mode: virtual blocks (doubled channel counts, pair_taps(k) taps) packed like any other block
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < 1; ++s) {
         st->pair_ok[s] = false;
         if (!(st->pair_mask & (1 << s)) || n < 2) continue;
         const int i = s == 0 ? 1 : 2 * n;
@@ -2549,7 +1910,6 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         pv.Npad = round_up(pv.cout, 16);
         pv.Ktot = round_up(pv.cin0, 64) + (pv.cin1 ? round_up(pv.cin1, 64) : 0);
         pv.mg_s = pv.mg_u = 0;
-        pv.tn_cp = pv.tn_npad = pv.tn_slots = pv.tn_groups = 0;
         const size_t nv = (size_t)pv.cout * (pv.cin0 + pv.cin1) * kp;
         const size_t nel = (size_t)kp * pv.Npad * pv.Ktot;
         if (!st->pair_w[s]) {
@@ -2567,34 +1927,6 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         if (cudaGetLastError() != cudaSuccess) return tc_fail("pack_tc_kernel (row-pair) launch failed");
         st->pair_ok[s] = true;
     }
-    return 0;
-}
-
-static int make_map_out(TcState *st, CUtensorMap *m, const void *base, uint64_t cout, uint64_t rows)
-{
-    cuuint64_t gdim[2] = {cout, rows};
-    cuuint64_t gstr[1] = {cout * 2};
-    cuuint32_t box[2] = {32, 32};
-    cuuint32_t estr[2] = {1, 1};
-    const CUresult r = st->encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), gdim, gstr, box, estr,
-                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return tc_fail("cuTensorMapEncodeTiled(out) failed (%d)", (int)r);
-    return 0;
-}
-
-// un-swizzled [d2][d1][d0] bf16 view with dense box rows (the head-only kernel's ring of previous-level rows)
-static int make_map_plain(TcState *st, CUtensorMap *m, const void *base, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b1)
-{
-    cuuint64_t gdim[3] = {d0, d1, d2};
-    cuuint64_t gstr[2] = {d0 * 2, d1 * d0 * 2};
-    cuuint32_t box[3] = {(cuuint32_t)d0, b1, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    const CUresult r = st->encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(base), gdim, gstr, box, estr,
-                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return tc_fail("cuTensorMapEncodeTiled(plain) failed (%d): dims %llu,%llu,%llu box rows %u", (int)r,
-                                          (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, b1);
     return 0;
 }
 
@@ -2722,14 +2054,8 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
     }
     // ---- tiling ---------------------------------------------------------------------------------
     TcOverride ov = parse_override(ovr, i);
-    if (pair && dec && !ov.any) parse_kv("mt=1,small=1", ov);      // fused head over row pairs: one epilogue warp per quadrant, resident weights
-    if (pair && !dec && !ov.any && B >= 128) parse_kv("mt=2,na=3", ov);   // block 1 over pairs, swept on a B200 at batch 256: 97 us (rules: 100)
-    if (!ov.any && B >= 128 && !sp)
-        for (const TunedTiling &t : kTuned)
-            if (t.L == L && t.cin0 == lv.cin0 && t.cin1 == lv.cin1 && t.cout == lv.cout && t.k == KS) parse_kv(t.kv, ov);
     const bool small = ov.small > 0 && !sp;
     const int smem_limit = small ? kSmemLimitSmall : kSmemLimit;
-    const int tmem_limit = small ? 256 : 512;
     P.small = small;
     const bool packed = L < 128 || (ov.packed > 0 && L + KS - 1 <= 256);
     auto geometry = [&](int MT, int nsplit) {
@@ -2763,45 +2089,26 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
             p.a_tx_bytes = FR * p.S * 128;
             p.m_tiles = (B + FR - 1) / FR;
         }
-        p.nacc = (ov.nacc != 1 && 2 * MT * p.Nstride <= tmem_limit) ? 2 : 1;
-        uint32_t cols = 32;
-        while ((int)cols < p.nacc * MT * p.Nstride) cols <<= 1;
-        p.tmem_cols = cols;
+        p.nacc = 1;
+        p.tmem_cols = 0;
     };
-    const int base_split = lv.Npad > 256 ? 2 : 1;
-    const int ns_sel = ov.ns > 0 ? ov.ns : base_split;
-    if (!packed) {
-        const int ns32 = round_up(ns_sel == 1 ? lv.Npad : round_up((lv.Npad + ns_sel - 1) / ns_sel, 16), 32);
-        int MT;
-        if (small) {
-            MT = ns32 <= 64 ? 2 : 1;       // 256 TMEM columns per CTA: double-buffered accumulators up to N = 128
-        } else if (ns32 <= 64) MT = 4;     // 2 x 4 x 64 TMEM columns: double-buffered accumulators (MT=2 measured 40 % slower on dec10/dec11)
-        else if (ns32 <= 96) MT = 2;       // 2 x 2 x 96
-        else if (ns32 <= 128) MT = 2;      // 2 x 2 x 128 columns: double-buffered accumulators beat the bigger MT=4 tile (73 vs 105 us on enc4)
-        else MT = dec ? 2 : 1;             // N > 128: encoders gain from double buffering at MT=1 (enc5: 60 vs 74 us); decoders do not
-        if (ov.mt > 0) MT = ov.mt;
-        if (hd_mt > 0 && small && i == 2 * n) MT = hd_mt;
-        while (MT > 1 && 128 * MT > L) --MT;
-        geometry(MT, ns_sel);
-    } else if (ov.mt > 0 || ov.ns > 0) {
-        geometry(ov.mt > 0 ? ov.mt : 1, ns_sel);
-    } else {
-        // bottom of the U: few tiles, long K loops. ONE wave of tiles (a second, partial wave costs a whole tile time:
-        // 172 tiles on 148 SMs measured 30-60 % slower than 129), the smallest M tile that allows it, and as many
-        // column splits as still fit in that wave (each CTA then streams a smaller share of the weights from L2).
-        int MT = 1, ns = base_split;
-        geometry(MT, ns);
-        while (p.m_tiles * ns > num_sms && MT < 4 && (MT + 1) * p.Nstride <= tmem_limit) geometry(++MT, ns);
+    // One 128-row M tile per CTA (MT = 1): the accumulators are registers of the consumer warpgroups, at most kAccColsLarge /
+    // kAccColsSmall columns per CTA, so wider blocks are split over CTAs by columns.
+    const int nh_max = small ? kAccColsSmall : kAccColsLarge;
+    int ns = std::max(ov.ns > 0 ? ov.ns : 1, (lv.Npad + nh_max - 1) / nh_max);
+    geometry(1, ns);
+    while (p.Nh > nh_max) geometry(1, ++ns);
+    if (packed && ov.ns <= 0) {
+        // bottom of the U: few tiles, long K loops. As many column splits as still fit in one wave of tiles (each CTA then
+        // streams a smaller share of the weights from L2).
         const int m_tiles = p.m_tiles;
         for (int cand : {2, 3, 4, 6}) {
             if (cand <= ns) continue;
             const int nh = round_up((lv.Npad + cand - 1) / cand, 16);
             if (m_tiles * cand <= num_sms && nh >= 48 && (cand - 1) * nh < lv.Npad) ns = cand;
         }
-        geometry(MT, ns);
+        geometry(1, ns);
     }
-    if ((int)p.tmem_cols > tmem_limit) return tc_fail("level %d: %u TMEM columns exceed %d", i, p.tmem_cols, tmem_limit);
-    if (p.Nh > 256) return tc_fail("level %d: N per CTA %d exceeds 256", i, p.Nh);
     if ((p.nsplit - 1) * p.Nh >= lv.Npad) return tc_fail("level %d: %d column splits of %d leave an empty split", i, p.nsplit, p.Nh);
     // epilogue store mode (needs complete tiles of complete rows per warp)
     p.bulk_store = 0;
@@ -2812,9 +2119,8 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
         // weights-resident mode: if the block's packed weights fit in shared memory next to the input ring, the persistent
         // CTA loads them once instead of re-streaming them from L2 for every tile (the L2->SM stream, not HBM and not the
         // tensor pipe, is what bounds the shallow blocks otherwise).
-        const int mt_pref = p.MT;
-        for (int MT = mt_pref; MT >= std::max(1, mt_pref / (dec ? 1 : 2)) && !p.resident; MT >>= 1) {
-            geometry(MT, 1);
+        {
+            geometry(1, 1);
             const int stage = round_up(p.Nh * 128 * KS, 1024);
             const int wbytes = p.nchunks * stage;
             const int na = ov.na > 0 ? ov.na : ((dec && p.nchunks >= 3) ? 3 : 2);
@@ -2824,7 +2130,7 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
                 p.nb = p.nchunks * p.ngroups;
             }
         }
-        if (!p.resident) geometry(mt_pref, 1);
+        if (!p.resident) geometry(1, 1);
     }
     if (!p.resident) {
         // A ring depth: decoders whose K chunks are short (5 taps, few K-steps) need the TMA/producers to run two chunks
@@ -2852,17 +2158,10 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
         if (!ok) return tc_fail("level %d does not fit in shared memory", i);
         if (ov.any && p.na < 2) return tc_fail("level %d: override leaves a single input stage", i);
     }
-    if (!sp && !packed && p.nsplit == 1 && ov.bulk != 0 && i != 2 * n && (L % (128 * p.MT) == 0) && (long long)B * L < (1LL << 31)) {
-        // TMA-store epilogue if the slabs fit without giving up ring depth / residency / tile size
-        const int need = p.n_epi * 2048 + 1024;
-        const int min_nb = p.resident ? p.nb : (p.tg == 1 ? 4 : 2);
-        while ((int)smem_total(p) + need > smem_limit && !p.resident && p.nb > min_nb) --p.nb;
-        if ((int)smem_total(p) + need <= smem_limit) p.bulk_store = 1;
-    }
     {
-        const int threads = 64 + 32 * (small ? kEpiWarpsSmall + (dec ? kProducerWarpsSmall : 0)
+        const int threads = 32 + 32 * (small ? kEpiWarpsSmall + (dec ? kProducerWarpsSmall : 0)
                                              : kEpiWarpsLarge + (dec ? kProducerWarpsLarge : 0));
-        const int per_sm = std::max(1, std::min({(int)((228 * 1024) / (smem_total(p) + 1024)), (int)(512 / p.tmem_cols), 2048 / threads}));
+        const int per_sm = std::max(1, std::min({(int)((228 * 1024) / (smem_total(p) + 1024)), small ? 2 : 1, 2048 / threads}));
         const int total_tiles = p.m_tiles * p.nsplit;
         p.tile_begin = 0; p.tile_end = total_tiles;
         P.per_sm = per_sm;
@@ -2874,7 +2173,6 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
 
     const bool last_block = (i == 2 * n);
     if (last_block && lv.cout > (pair ? 64 : 32)) return tc_fail("fused head needs channels_interval <= 32");
-    if (last_block && pair && (!small || p.MT > 2)) return tc_fail("row-pair head needs the small flavour and MT <= 2");
     if (dec && pair && p.na < p.nchunks0) return tc_fail("level %d: the row-pair producers fill %d ring stages at once, the ring has %d", i, p.nchunks0, p.na);
     if (last_block && p.packed) return tc_fail("bf16 path needs frames of at least 128 samples (T=%d): the fused head works on full frames", T);
     if (last_block && p.nsplit != 1) return tc_fail("fused head needs the whole channel range in one CTA");
@@ -2897,7 +2195,7 @@ static bool plan_block_gemm(const TcLevel &lv, int i, int n, int B, int T, int n
     // columns per CTA: a multiple of 16 that divides N, giving about one CTA per SM (times the 256-frame row tiles)
     const int mtiles = (B + 127) / 128;
     int best = 16;
-    for (int nh = 16; nh <= 256; nh += 16)
+    for (int nh = 16; nh <= kAccColsLarge; nh += 16)
         if (g.N % nh == 0 && (g.N / nh) * mtiles >= num_sms * 3 / 4) best = nh;
     g.Nh = best;
     const int pad = (lv.k - 1) / 2;
@@ -2914,92 +2212,16 @@ static bool plan_block_gemm(const TcLevel &lv, int i, int n, int B, int T, int n
     int ns = (kSmemLimit - 2048) / (int)(g.cps * (g.a_bytes + g.w_bytes));
     while (ns < 2 && g.cps > 1) { --g.cps; ns = (kSmemLimit - 2048) / (int)(g.cps * (g.a_bytes + g.w_bytes)); }
     g.nstages = std::min(4, std::max(2, ns));
-    uint32_t cols = 32;
-    while ((int)cols < g.Nh) cols <<= 1;
-    g.tmem_cols = cols;
-    P.is_gemm = true; P.upcat = dec; P.small = false; P.per_sm = 1; P.threads = 192;
+    P.is_gemm = true; P.upcat = dec; P.small = false; P.per_sm = 1; P.threads = kGemmThreads;
     P.kind = 2;
-    P.smem = (size_t)g.nstages * g.cps * (g.a_bytes + g.w_bytes) + 8 * 20 + 1024;
+    P.smem = (size_t)g.nstages * g.cps * (g.a_bytes + g.w_bytes) + 8 * 16 + 1024;
     P.grid = dim3((unsigned)(g.N / g.Nh), (unsigned)mtiles, 1);
     TcParams &p = P.p;                                          // mirror what tests / tools read
     memset(&p, 0, sizeof(p));
     p.B = B; p.L = L; p.T = T; p.Cout = lv.cout; p.Cin0 = lv.cin0; p.Cin1 = lv.cin1; p.Npad = lv.Npad; p.Nh = g.Nh; p.nsplit = g.N / g.Nh;
     p.Nstride = g.Nh; p.MT = 1; p.nacc = 1; p.FR = 128; p.packed = 1; p.S = L; p.m_tiles = mtiles; p.nchunks = g.npos[0] * g.cpp[0] + g.npos[1] * g.cpp[1];
     p.na = g.nstages; p.nb = g.nstages; p.tg = 1; p.ngroups = 1; p.a_stage_bytes = g.cps * g.a_bytes; p.b_stage_bytes = g.cps * g.w_bytes;
-    p.a_tx_bytes = (int)(g.cps * g.a_bytes); p.rows_used = 128; p.tmem_cols = cols; p.tile_begin = 0; p.tile_end = p.m_tiles * p.nsplit; p.n_epi = 4;
-    return true;
-}
-
-// Tiling of a taps-in-N block (conv_tn_kernel): pure host logic like plan_block. Returns false if the block does not take
-// this path at this shape (frames shorter than a tile, channel plan not eligible).
-static bool plan_block_tn(const TcLevel &lv, int i, int n, int B, int T, int num_sms, TcPlanLevel &P)
-{
-    if (!lv.tn_slots) return false;
-    const bool dec = i > n;
-    const int L = (i <= n) ? (T >> i) : (T >> (2 * n - i));
-    const bool last = (i == 2 * n);
-    TnParams &t = P.tn;
-    memset(&t, 0, sizeof(t));
-    t.Cout = lv.cout; t.Cp = lv.tn_cp; t.Npad = lv.tn_npad; t.Nstride = round_up(t.Npad, 32);
-    int MT = 512 / (2 * t.Nstride);                                   // double-buffered accumulators
-    if (MT > 4) MT = 4;
-    if (MT < 1) return false;
-    if (last && MT < 2) return false;                                 // the fused head splits the sub-tiles between warp pairs
-    if (L < 112 * MT * 2) return false;                               // long blocks only
-    t.B = B; t.L = L; t.T = T; t.MT = MT; t.tile_rows = 112 * MT;
-    t.tiles_per_frame = (L + t.tile_rows - 1) / t.tile_rows;
-    t.Cin0 = lv.cin0; t.Cin1 = lv.cin1; t.pad = (lv.k - 1) / 2;
-    int k = 0;
-    auto add = [&](int up, int ch, int cwidth, int slot, int row) {
-        t.c_up[k] = (unsigned char)up; t.c_ch[k] = (unsigned char)ch; t.c_nk[k] = (unsigned char)((std::min(cwidth, 64) + 15) / 16);
-        t.c_slot[k] = (unsigned char)slot; t.c_row[k] = (unsigned char)row; ++k;
-    };
-    if (dec) {
-        // K-loop order as in conv_tc_kernel: full upsampled chunks, skip chunks (TMA), then the partial upsampled chunk; if the
-        // only upsampled chunk is partial it goes first
-        const int n0 = (lv.cin0 + 63) / 64, n1 = (lv.cin1 + 63) / 64, nfull0 = lv.cin0 / 64;
-        if (nfull0 == 0) add(1, 0, lv.cin0, 0, 0);
-        for (int c = 0; c < nfull0; ++c) add(1, c, 64, c, 0);
-        for (int c = 0; c < n1; ++c) add(0, c, lv.cin1 - 64 * c, n0 + c, 0);
-        if (nfull0 > 0 && nfull0 < n0) add(1, nfull0, lv.cin0 - 64 * nfull0, nfull0, 0);
-    } else {
-        for (int g = 0; g < lv.tn_groups; ++g) add(0, 0, lv.cin0, g, 5 * g);
-    }
-    t.nchunks = k;
-    t.a_sub_bytes = (uint32_t)(MT * 4 * 4096);
-    t.a_stage_bytes = (uint32_t)t.nchunks * t.a_sub_bytes;
-    t.w_tile_bytes = (uint32_t)round_up(t.Npad * 128, 1024);
-    const int budget = kSmemLimit - 2048 - t.Cout * 8 - 512 - t.nchunks * (int)t.w_tile_bytes;
-    int na = budget / (int)t.a_stage_bytes;
-    if (na > 4) na = 4;
-    if (const char *e = getenv("WUNET_TN_NA")) na = std::min(na, std::max(2, atoi(e)));
-    if (na < 2) return false;
-    t.na = na;
-    t.tmem_cols = 512;
-    // producer groups: enough warps per group to give every thread at most one item of the widest upsampled chunk
-    int items = 0;
-    for (int c = 0; c < t.nchunks; ++c) {
-        if (t.c_up[c]) items += 8 * MT * 2 * (int)t.c_nk[c];
-        else ++t.ntma;
-    }
-    t.nup_items = items;
-    t.wpg = std::max(1, std::min(kProducerWarpsLarge, (items + 31) / 32));
-    t.npg = std::max(1, kProducerWarpsLarge / t.wpg);
-    t.head = last ? 1 : 0;
-    const int total_tiles = B * t.tiles_per_frame;
-    t.tile_begin = 0; t.tile_end = total_tiles;
-    P.is_tn = true; P.upcat = dec; P.small = false; P.per_sm = 1;
-    P.threads = 64 + 32 * (kEpiWarpsLarge + (dec ? kProducerWarpsLarge : 0));
-    P.smem = tn_smem_total(t);
-    P.grid = dim3((unsigned)std::min(total_tiles, num_sms), 1, 1);
-    // mirror the fields tests / tools read from TcParams
-    TcParams &p = P.p;
-    memset(&p, 0, sizeof(p));
-    p.B = B; p.L = L; p.T = T; p.Cout = lv.cout; p.Cin0 = lv.cin0; p.Cin1 = lv.cin1; p.Npad = t.Npad; p.Nh = t.Npad; p.nsplit = 1;
-    p.Nstride = t.Nstride; p.MT = MT; p.nacc = 2; p.FR = 1; p.m_tiles = total_tiles; p.nchunks = t.nchunks; p.resident = 1;
-    p.na = na; p.nb = t.nchunks; p.tg = 5; p.ngroups = 1; p.a_stage_bytes = t.a_stage_bytes; p.b_stage_bytes = t.w_tile_bytes;
-    p.a_tx_bytes = (int)t.a_stage_bytes; p.rows_used = 128 * MT; p.tmem_cols = 512; p.tiles_per_frame = t.tiles_per_frame;
-    p.tile_begin = 0; p.tile_end = total_tiles; p.n_epi = kEpiWarpsLarge;
+    p.a_tx_bytes = (int)(g.cps * g.a_bytes); p.rows_used = 128; p.tmem_cols = 0; p.tile_begin = 0; p.tile_end = p.m_tiles * p.nsplit; p.n_epi = kEpiWarpsLarge;
     return true;
 }
 
@@ -3027,8 +2249,7 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
         p.x = x; p.y = y; p.head_w = st->out_w; p.head_b = st->out_b; p.trace = nullptr;
         __nv_bfloat16 *xb = reinterpret_cast<__nv_bfloat16 *>(base + pl.off[2 * n + 2]);
         if (make_map(st, &P.tmA, xb, 8, L, B, (uint64_t)8 * 2, (uint64_t)L * 8 * 2, 64, (uint32_t)p.R1, 1u)) return -1;
-        if (p.bulk_store) { if (make_map_out(st, &P.tmO, p.out, (uint64_t)lv.cout, (uint64_t)B * L)) return -1; }
-        else P.tmO = P.tmA;
+        P.tmO = P.tmA;
         p.hd = 0; p.ps_n = 0; p.ps_rows = p.ps_rows2 = 0; p.ps_bytes = 0; p.ps_tx = p.ps_tx2 = 0;
         if (make_map(st, &P.tmW, lv.wp, (uint64_t)lv.Ktot, lv.Npad, lv.k, (uint64_t)lv.Ktot * 2, (uint64_t)lv.Npad * lv.Ktot * 2, 64, (uint32_t)p.Nh,
                      (uint32_t)p.tg))
@@ -3037,10 +2258,10 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
     }
     for (int i = 1; i < 2 * n + 1; ++i) {
         // row-pair mode (WUNET_TC_PAIR): block 1 and / or the last block run as virtual blocks over pairs of positions
-        const int ps = (n >= 2 && i == 1) ? 0 : ((n >= 2 && i == 2 * n) ? 1 : -1);
+        const int ps = (n >= 2 && i == 1) ? 0 : -1;
         const int Lreal = (i <= n) ? (T >> i) : (T >> (2 * n - i));
-        const bool pair = ps >= 0 && !sp && st->pair_ok[ps] && Lreal % 2 == 0 && Lreal / 2 >= 128 && !st->tn &&
-                          !(ps == 1 && st->headk) && !(ps == 0 && pl.enc0_tc);      // the even-row copy comes from the CUDA-core enc0
+        const bool pair = ps >= 0 && !sp && st->pair_ok[ps] && Lreal % 2 == 0 && Lreal / 2 >= 128 &&
+                          !pl.enc0_tc;      // the even-row copy comes from the CUDA-core enc0
         const TcLevel &lv = pair ? st->pair_lv[ps] : st->levels[i];
         TcPlanLevel &P = pl.lv[i];
         if (!pair && !sp && st->gemm && parse_override(st->plan_ovr, i).any == false && plan_block_gemm(lv, i, n, B, T, st->num_sms, P)) {
@@ -3075,31 +2296,7 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
                 return -1;
             continue;
         }
-        if (!pair && !sp && parse_override(st->plan_ovr, i).any == false && plan_block_tn(lv, i, n, B, T, st->num_sms, P)) {
-            TnParams &t = P.tn;
-            const bool dec = i > n;
-            const bool last = (i == 2 * n);
-            t.ss = lv.ss;
-            t.out = (last && !st->store_last) ? nullptr : lvl(i);
-            t.head_w = st->out_w; t.head_b = st->out_b;
-            if (!dec) {
-                const int Cp = lv.cin0, Lp = 2 * t.L;           // decimated view of the previous encoder output (o[:, :, ::2])
-                if (make_map(st, &P.tmA, lvl(i - 1), Cp, t.L, B, (uint64_t)2 * Cp * 2, (uint64_t)Lp * Cp * 2, 64, 32, 1)) return -1;
-            } else {
-                const int e = 2 * n - i, Cs = lv.cin1;
-                if (make_map(st, &P.tmA, lvl(e), Cs, t.L, B, (uint64_t)Cs * 2, (uint64_t)t.L * Cs * 2, 64, 32, 1)) return -1;
-                t.prev = lvl(i - 1);
-                t.Lin = t.L / 2;
-                t.up_scale = (t.L > 1) ? (float)(t.Lin - 1) / (float)(t.L - 1) : 0.f;
-            }
-            if (make_map(st, &P.tmW, lv.wp_tn, (uint64_t)lv.tn_slots * 64, (uint64_t)lv.tn_npad, 1, (uint64_t)lv.tn_slots * 128,
-                         (uint64_t)lv.tn_npad * lv.tn_slots * 128, 64, (uint32_t)lv.tn_npad, 1))
-                return -1;
-            P.tmO = P.tmA;
-            continue;
-        }
-        const bool hd_want = (i == 2 * n) && !st->store_last && !sp && st->headk && !pair;
-        if (plan_block(lv, i, n, B, T, st->num_sms, st->plan_ovr, P, sp, hd_want ? st->head_mt : 0, pair)) return -1;
+        if (plan_block(lv, i, n, B, T, st->num_sms, st->plan_ovr, P, sp, 0, pair)) return -1;
         TcParams &p = P.p;
         const bool dec = i > n;
         const int L = p.L;
@@ -3130,31 +2327,8 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
             p.Lin = pair ? L : L / 2;                         // row-pair mode: an operand row IS a previous-level row index
             p.up_scale = pair ? (float)(p.Lin - 1) / (float)(2 * L - 1) : ((L > 1) ? (float)(p.Lin - 1) / (float)(L - 1) : 0.f);
         }
-        if (p.out != nullptr && !sp) { if (make_map_out(st, &P.tmO, p.out, (uint64_t)lv.cout, (uint64_t)B * L)) return -1; }
-        else P.tmO = P.tmA;
+        P.tmO = P.tmA;
         p.hd = 0; p.ps_n = 0; p.ps_rows = p.ps_rows2 = 0; p.ps_bytes = 0; p.ps_tx = p.ps_tx2 = 0;
-        if (last && dec && p.out == nullptr && !sp && P.small && !p.mg && !p.packed && !p.bulk_store && p.resident && p.Npad <= 32 &&
-            p.Nh == p.Npad && p.MT <= 4 && lv.cin0 % 8 == 0 && lv.cin1 % 8 == 0 && p.nchunks == 2 && (p.chunk_map[0] & 0x80) &&
-            !(p.chunk_map[1] & 0x80) && st->headk) {
-            // head-only instantiation (conv_tc_kernel<..., HD = 1>): both operand chunks are producer-written from a ring of
-            // [previous-level window | skip rows] entries; as many slots (3..8) as still leave two CTAs per SM
-            // output row j of the tile interpolates between window rows (j >> 1) + (j & 1) and that + 1 (the producers clamp the
-            // index for the masked rows past rows_used of their last item)
-            const int rows = ((p.rows_used + 1) >> 1) + 2, rows2 = p.rows_used;
-            if (rows <= 256 && rows2 <= 256 && p.Lin >= rows && L >= rows2) {
-                p.ps_rows = rows; p.ps_rows2 = rows2;
-                p.ps_tx = (uint32_t)rows * (uint32_t)lv.cin0 * 2u;
-                p.ps_tx2 = (uint32_t)rows2 * (uint32_t)lv.cin1 * 2u;
-                p.ps_bytes = (uint32_t)round_up((int)std::max(p.ps_tx, p.ps_tx2), 128);
-                for (p.ps_n = 8; p.ps_n >= 3 && (int)smem_total(p) > kSmemLimitSmall; --p.ps_n) { }
-                if (p.ps_n >= 3) {
-                    p.hd = 1;
-                    P.smem = smem_total(p);
-                    if (make_map_plain(st, &P.tmO, lvl(i - 1), (uint64_t)lv.cin0, (uint64_t)p.Lin, (uint64_t)B, (uint32_t)rows)) return -1;
-                    if (make_map_plain(st, &P.tmA, lvl(2 * n - i), (uint64_t)lv.cin1, (uint64_t)L, (uint64_t)B, (uint32_t)rows2)) return -1;
-                } else p.ps_n = 0;
-            }
-        }
         const uint64_t ktot = sp ? (uint64_t)lv.sp_chunks * 64 : (uint64_t)lv.Ktot;
         if (make_map(st, &P.tmW, sp ? lv.wp_sp : lv.wp, ktot, lv.Npad, lv.k, ktot * 2, (uint64_t)lv.Npad * ktot * 2, 64,
                      (uint32_t)p.Nh, (uint32_t)p.tg))
@@ -3167,12 +2341,6 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
                 const GemmParams &g = pl.lv[i].gp;
                 fprintf(stderr, "[wunet gemm] blk %2d L=%2d N=%5d Nh=%3d K chunks=%d+%d stages=%d x %d chunks grid=%ux%u smem=%zu\n", i, g.L, g.N, g.Nh,
                         g.npos[0] * g.cpp[0], g.npos[1] * g.cpp[1], g.nstages, g.cps, pl.lv[i].grid.x, pl.lv[i].grid.y, pl.lv[i].smem);
-                continue;
-            }
-            if (pl.lv[i].is_tn) {
-                const TnParams &t = pl.lv[i].tn;
-                fprintf(stderr, "[wunet tn] blk %2d L=%5d Cin=%3d+%3d Cout=%3d N'=%3d MT=%d chunks=%d na=%d wpg=%d npg=%d smem=%zu tiles=%d grid=%u\n", i, t.L,
-                        t.Cin0, t.Cin1, t.Cout, t.Npad, t.MT, t.nchunks, t.na, t.wpg, t.npg, pl.lv[i].smem, t.tile_end, pl.lv[i].grid.x);
                 continue;
             }
             fprintf(stderr, "[wunet tc] blk %2d L=%5d Cin=%3d+%3d Cout=%3d Nh=%3d x%d MT=%d nacc=%d packed=%d FR=%d res=%d bulk=%d na=%d nb=%d tg=%d smem=%zu tmem=%u tiles=%d grid=%u small=%d per_sm=%d hd=%d ring=%d\n",
@@ -3189,7 +2357,7 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
     const char *e0 = getenv("WUNET_TC_ENC0");
     const bool g8 = block == 0 && e0 && e0[0] == '1';        // block 0 has a tensor-core plan only in its group-of-8 form
     if (nblocks != 2 * n + 1 || (block < 1 && !g8) || block >= nblocks) return tc_fail("block %d out of range (1..%d)", block, 2 * n);
-    if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tcgen05 path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
+    if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
     if (cap < 32 || !f) return tc_fail("need room for 32 fields");
     if (g8) {
         if (blocks[0].k != 15 || blocks[0].cin != 1 || 8 * blocks[0].cout > 256 || T % 8 != 0 || T / 8 < 128) return tc_fail("block 0 has no group-of-8 plan for this shape");
@@ -3208,43 +2376,36 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
     }
     std::vector<TcLevel> levels(nblocks);
     const char *mge = getenv("WUNET_TC_MERGE");
-    const char *tne = getenv("WUNET_TC_TN");
-    derive_levels(levels, blocks, nblocks, n, !(mge && mge[0] == '0'), tne && tne[0] == '1');
+    derive_levels(levels, blocks, nblocks, n, !(mge && mge[0] == '0'));
     const char *ovr = getenv("WUNET_TC_OVR");
     TcPlanLevel P{};
     const std::string ovr_s = ovr ? ovr : "";
     const char *ge = getenv("WUNET_TC_GEMM");
     bool planned = false;
     {
-        // row-pair mode (WUNET_TC_PAIR bit 0: block 1, bit 1: last block), planned like build_plan does
-        const char *pe = getenv("WUNET_TC_PAIR"), *hk = getenv("WUNET_TC_HEADK");
-        const int pmask = pe ? atoi(pe) & 3 : 1;
-        const int ps = (n >= 2 && block == 1) ? 0 : ((n >= 2 && block == 2 * n) ? 1 : -1);
+        // row-pair mode of block 1 (WUNET_TC_PAIR bit 0), planned like build_plan does
+        const char *pe = getenv("WUNET_TC_PAIR");
+        const int pmask = pe ? atoi(pe) & 1 : 1;
+        const int ps = (n >= 2 && block == 1) ? 0 : -1;
         const int Lreal = (block <= n) ? (T >> block) : (T >> (2 * n - block));
-        if (ps >= 0 && (pmask & (1 << ps)) && Lreal % 2 == 0 && Lreal / 2 >= 128 && !(tne && tne[0] == '1') && !(ps == 1 && hk && hk[0] == '1')) {
+        if (ps >= 0 && (pmask & (1 << ps)) && Lreal % 2 == 0 && Lreal / 2 >= 128) {
             const TcLevel &rl = levels[block];
-            const bool ok = ps == 0 ? (rl.k == 15 && rl.cin1 == 0 && rl.cin0 % 8 == 0 && 2 * rl.cin0 <= 64 && 2 * rl.cout <= 256)
-                                    : (rl.k == 5 && rl.cin0 % 8 == 0 && rl.cin1 % 8 == 0 && rl.cin0 >= 32 && rl.cout % 8 == 0 && rl.cout <= 32);
+            const bool ok = rl.k == 15 && rl.cin1 == 0 && rl.cin0 % 8 == 0 && 2 * rl.cin0 <= 64 && 2 * rl.cout <= 256;
             if (ok) {
                 TcLevel pv = rl;
                 pv.cin0 = 2 * rl.cin0; pv.cin1 = 2 * rl.cin1; pv.cout = 2 * rl.cout; pv.k = pair_taps(rl.k);
                 pv.Npad = round_up(pv.cout, 16);
                 pv.Ktot = round_up(pv.cin0, 64) + (pv.cin1 ? round_up(pv.cin1, 64) : 0);
-                pv.mg_s = pv.mg_u = 0; pv.tn_slots = 0;
+                pv.mg_s = pv.mg_u = 0;
                 if (plan_block(pv, block, n, B, T, num_sms, ovr_s, P, false, 0, true)) return -1;
                 planned = true;
             }
         }
     }
-    if (planned) {
-    } else if (!(ge && ge[0] == '0') && parse_override(ovr_s, block).any == false && plan_block_gemm(levels[block], block, n, B, T, num_sms, P)) {
-    } else if (!(parse_override(ovr_s, block).any == false && plan_block_tn(levels[block], block, n, B, T, num_sms, P))) {
-        // the last block as the forward plans it by default (head-only instantiation unless WUNET_TC_STORE_LAST=1 / WUNET_TC_HEADK=0)
-        const char *sl = getenv("WUNET_TC_STORE_LAST"), *hk = getenv("WUNET_TC_HEADK"), *hm = getenv("WUNET_TC_HEADMT");
-        const bool hd_want = block == 2 * n && !(sl && sl[0] == '1') && (hk && hk[0] == '1');
-        const int head_mt = hm ? std::max(1, std::min(4, atoi(hm))) : 1;
-        if (plan_block(levels[block], block, n, B, T, num_sms, ovr_s, P, false, hd_want ? head_mt : 0)) return -1;
-    }
+    if (!planned && !(!(ge && ge[0] == '0') && parse_override(ovr_s, block).any == false &&
+                      plan_block_gemm(levels[block], block, n, B, T, num_sms, P)) &&
+        plan_block(levels[block], block, n, B, T, num_sms, ovr_s, P, false, 0))
+        return -1;
     const TcParams &p = P.p;
     const int v[32] = {p.L, p.Cin0, p.Cin1, p.Cout, p.Npad, p.Nh, p.nsplit, p.Nstride, p.MT, p.nacc, p.packed, p.FR, p.S, p.m_tiles,
                        p.nchunks, p.resident, p.bulk_store, p.na, p.nb, p.tg, p.ngroups, (int)p.a_stage_bytes, (int)p.b_stage_bytes,
@@ -3258,7 +2419,7 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
 {
     if (!st) return tc_fail("tensor-core state missing");
     const int ci = st->ci;
-    if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tcgen05 path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
+    if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
     if (!st->attr_set) {
         cudaFuncSetAttribute(conv_tc_kernel<15, false, kEpiWarpsLarge, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
@@ -3266,21 +2427,13 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
         cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsSmall, kProducerWarpsSmall, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsSmall, kProducerWarpsSmall, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
-        cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsSmall, kProducerWarpsSmall, 0, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<15, false, kEpiWarpsLarge, 0, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<3, false, kEpiWarpsLarge, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<3, false, kEpiWarpsSmall, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<9, false, kEpiWarpsLarge, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<9, false, kEpiWarpsSmall, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
-        cudaFuncSetAttribute(conv_tc_kernel<3, true, kEpiWarpsSmall, kProducerWarpsSmall, 0, 0, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
-        cudaFuncSetAttribute(conv_tn_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
-        cudaFuncSetAttribute(conv_tn_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
-#ifdef WUNET_TN_DEBUG
-#define TN_ATTR(D) cudaFuncSetAttribute(conv_tn_kernel<true, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit); cudaFuncSetAttribute(conv_tn_kernel<false, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
-        TN_ATTR(1) TN_ATTR(2) TN_ATTR(4) TN_ATTR(8) TN_ATTR(16) TN_ATTR(32) TN_ATTR(3) TN_ATTR(7) TN_ATTR(24) TN_ATTR(56) TN_ATTR(63)
-#endif
         cudaFuncSetAttribute(enc0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         cudaFuncSetAttribute(enc0_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         int dev = 0, sms = 0;
@@ -3311,7 +2464,7 @@ static int launch_enc0(TcState *st, const float *x, int f0, int nf, int T, void 
         const long long n4 = (long long)nf * T / 4;
         x_to_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(x + (size_t)f0 * T, xb, n4);
         if (cudaGetLastError() != cudaSuccess) return tc_fail("x_to_bf16_kernel launch failed");
-        const int tpf = st->plan.lv[0].p.tiles_per_frame;
+        const int tpf = st->plan.lv[0].p.tiles_per_frame * st->plan.lv[0].p.nsplit;    // tiles of one frame, all column splits
         if (launches) *launches = 2;
         return launch_block(st, 0, f0 * tpf, (f0 + nf) * tpf, stream, nullptr, nullptr);
     }
@@ -3358,33 +2511,6 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
         if (e != cudaSuccess) return tc_fail("gemm_tc level %d launch failed: %s", i, cudaGetErrorString(e));
         return 0;
     }
-    if (P.is_tn) {
-        TnParams t = P.tn;
-        t.x = x; t.y = y;
-        if (t1 >= 0) { t.tile_begin = t0; t.tile_end = t1; }
-        const int ntiles = t.tile_end - t.tile_begin;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3((unsigned)std::min(ntiles, st->num_sms), 1, 1);
-        cfg.blockDim = dim3(P.threads); cfg.dynamicSmemBytes = P.smem; cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = st->pdl ? 1 : 0;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-#ifdef WUNET_TN_DEBUG
-#define TN_CASE(D) case D: if (P.upcat) cudaLaunchKernelEx(&cfg, conv_tn_kernel<true, D>, P.tmA, P.tmW, t); else cudaLaunchKernelEx(&cfg, conv_tn_kernel<false, D>, P.tmA, P.tmW, t); break;
-        if (const char *de = getenv("WUNET_TN_DBG")) t.dbg = atoi(de);
-        switch (t.dbg) { TN_CASE(1) TN_CASE(2) TN_CASE(4) TN_CASE(8) TN_CASE(16) TN_CASE(32) TN_CASE(3) TN_CASE(7) TN_CASE(24) TN_CASE(56) TN_CASE(63)
-        default:
-#endif
-        if (P.upcat) cudaLaunchKernelEx(&cfg, conv_tn_kernel<true, 0>, P.tmA, P.tmW, t);
-        else cudaLaunchKernelEx(&cfg, conv_tn_kernel<false, 0>, P.tmA, P.tmW, t);
-#ifdef WUNET_TN_DEBUG
-        }
-#endif
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return tc_fail("conv_tn level %d launch failed: %s", i, cudaGetErrorString(e));
-        return 0;
-    }
     TcParams p = P.p;
     p.x = x; p.y = y;                                    // only the fused head (last block) reads x / writes y
     p.pf_late = st->pf_late ? 1 : 0;
@@ -3405,15 +2531,9 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
         // row-pair mode of the first tensor-core encoder block: a 9-tap block over pairs of positions
         if (!P.small) cudaLaunchKernelEx(&cfg, conv_tc_kernel<9, false, kEpiWarpsLarge, 0, 0>, P.tmA, P.tmW, P.tmO, p);
         else cudaLaunchKernelEx(&cfg, conv_tc_kernel<9, false, kEpiWarpsSmall, 0, 0>, P.tmA, P.tmW, P.tmO, p);
-    } else if (P.pair == 2) {
-        // row-pair mode of the last decoder block + head: 3 taps over pairs, producers and head in their PR = 1 form
-        cudaLaunchKernelEx(&cfg, conv_tc_kernel<3, true, kEpiWarpsSmall, kProducerWarpsSmall, 0, 0, 0, 1>, P.tmA, P.tmW, P.tmO, p);
     } else if (p.split) {
         if (P.upcat) cudaLaunchKernelEx(&cfg, conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 0, 1>, P.tmA, P.tmW, P.tmO, p);
         else cudaLaunchKernelEx(&cfg, conv_tc_kernel<15, false, kEpiWarpsLarge, 0, 0, 1>, P.tmA, P.tmW, P.tmO, p);
-    } else if (p.hd) {
-        // last decoder block, only the network output wanted: head-only instantiation
-        cudaLaunchKernelEx(&cfg, conv_tc_kernel<5, true, kEpiWarpsSmall, kProducerWarpsSmall, 0, 0, 1>, P.tmA, P.tmW, P.tmO, p);
     } else if (P.upcat && p.mg) {
         if (!P.small) cudaLaunchKernelEx(&cfg, conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 1>, P.tmA, P.tmW, P.tmO, p);
         else cudaLaunchKernelEx(&cfg, conv_tc_kernel<5, true, kEpiWarpsSmall, kProducerWarpsSmall, 1>, P.tmA, P.tmW, P.tmO, p);
@@ -3553,7 +2673,7 @@ void tc_destroy(TcState *st)
         }
         cudaFree(st->trace);
     }
-    for (auto &lv : st->levels) { cudaFree(lv.wp); cudaFree(lv.ss); cudaFree(lv.w_own); cudaFree(lv.wp_tn); cudaFree(lv.wp_sp); cudaFree(lv.w_f32); cudaFree(lv.wx); }
+    for (auto &lv : st->levels) { cudaFree(lv.wp); cudaFree(lv.ss); cudaFree(lv.w_own); cudaFree(lv.wp_sp); cudaFree(lv.w_f32); cudaFree(lv.wx); }
     cudaFree(st->g8_lv.wp); cudaFree(st->g8_lv.ss); cudaFree(st->g8_w); cudaFree(st->g8_scale); cudaFree(st->g8_shift);
     for (int s = 0; s < 2; ++s) { cudaFree(st->pair_lv[s].wp); cudaFree(st->pair_lv[s].ss); cudaFree(st->pair_w[s]); cudaFree(st->pair_scale[s]); cudaFree(st->pair_shift[s]); }
     delete st;

@@ -1,4 +1,4 @@
-// wunet_tc.cuh — interface of the bf16 / tcgen05 tensor-core path (implemented in wunet_tc.cu).
+// wunet_tc.cuh — interface of the bf16 / wgmma tensor-core path (implemented in wunet_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

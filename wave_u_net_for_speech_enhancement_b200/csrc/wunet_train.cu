@@ -1,6 +1,6 @@
 // wunet_train.cu — training step of the Wave-U-Net (SURVEY.md §8f row N1): forward with BatchNorm1d in training mode and the
-// backward pass, fp32, NCL layout, CUDA cores (one formula per kernel, in the order autograd would replay them); validated on a
-// B200 against float64 golden steps (tests/test_train_gpu.py). The three convolution-shaped passes carry ~99 % of the work:
+// backward pass, fp32, NCL layout, CUDA cores (one formula per kernel, in the order autograd would replay them); checked
+// against float64 golden steps (tests/test_train_gpu.py). The three convolution-shaped passes carry ~99 % of the work:
 //   forward conv and input gradient  -> the tuned fp32 kernels of wunet_fp32.cu (sliding-window / implicit GEMM) with a linear
 //                                       epilogue; the input gradient is the same convolution with the weights transposed and
 //                                       flipped, read from dz (train_pack_kernel writes both packings every step);

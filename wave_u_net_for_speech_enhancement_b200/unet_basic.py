@@ -1,5 +1,5 @@
 """
-Drop-in replacement for the reference's ``model/unet_basic.py`` (``Model``), forward path on B200.
+Drop-in replacement for the reference's ``model/unet_basic.py`` (``Model``), forward path on H100.
 
 Selected through the reference's own plugin loader (``util/utils.py:55-72``) by changing ONLY the
 ``"module"`` string of the ``"model"`` stanza (``config/train/train.json:22-26``)::
@@ -16,7 +16,7 @@ Surface kept identical to the reference (SURVEY §8b):
 
 The sub-modules below exist ONLY as parameter/buffer containers with the reference's names; their
 ``forward`` is never called on the product path.  ``Model.forward`` hands device pointers to the
-hand-written sm_100a kernels in ``libwunet_b200.so`` through the C ABI (``include/wunet_b200.h``).
+hand-written sm_90a kernels in ``libwunet_b200.so`` through the C ABI (``include/wunet_b200.h``).
 There is no CPU or PyTorch fallback for the eval forward: a CPU tensor or a missing library raises.
 """
 from __future__ import annotations
@@ -202,18 +202,18 @@ class _NativeTrainStep(torch.autograd.Function):
 
 
 class Model(nn.Module):
-    """Wave-U-Net whose eval forward runs on hand-written sm_100a kernels.
+    """Wave-U-Net whose eval forward runs on hand-written sm_90a kernels.
 
     Extra keyword arguments (not in the reference; configs pass ``"args": {}`` so defaults apply):
 
-    precision      "fp32_tc" (default): fp32-grade results on the tensor cores (bf16 hi + lo split, three tcgen05 MMAs per
+    precision      "fp32_tc" (default): fp32-grade results on the tensor cores (bf16 hi + lo split, three MMAs per
                    product; <=1e-4 vs the reference, measured 1e-6; needs channels_interval % 8 == 0 and <= 32);
-                   "fp32": the same contract on CUDA-core FFMA for any channel plan (12x slower);
-                   "bf16": bf16 activations / operands on tcgen05 (the fastest path; ~6e-4 on the output).
+                   "fp32": the same contract on CUDA-core FFMA for any channel plan (slower);
+                   "bf16": bf16 activations / operands on the tensor cores (the fastest path; ~6e-4 on the output).
     train_backend  "native" (default): a forward in training mode runs ``wunet_train_forward`` (BatchNorm with batch
                    statistics, running buffers updated) behind a ``torch.autograd.Function`` whose backward is
                    ``wunet_train_backward_part``; the reference's loss, ``loss.backward()`` and optimizer run unchanged
-                   (trainer/trainer.py:34-38). fp32, validated against float64 golden steps on a B200.
+                   (trainer/trainer.py:34-38). fp32, checked against float64 golden steps.
                    "torch": opt-in composite of torch ops with the reference's semantics (runs on CPU too), used by the
                    CPU boundary tests that drive the unchanged ``trainer/trainer.py`` loop; not a measured hot path.
                    "none": a forward in training mode raises NotImplementedError.
@@ -321,7 +321,7 @@ class Model(nn.Module):
                 return self._forward_train_native(input)
             raise NotImplementedError(
                 "this model was built with train_backend='none': call model.eval(), or construct it with "
-                "train_backend='native' (default; sm_100a kernels) or 'torch' (composite PyTorch path).")
+                "train_backend='native' (default; sm_90a kernels) or 'torch' (composite PyTorch path).")
         # eval mode: like enhancement.py:66 (`model(chunk).detach().cpu()`, no torch.no_grad()) the result is
         # returned detached — the native path records no autograd graph.
         return self._forward_native(input)
@@ -341,7 +341,7 @@ class Model(nn.Module):
         self._check_input(x)
         if not x.is_cuda:
             raise RuntimeError("wave_u_net_for_speech_enhancement_b200 has no CPU fallback: move the model and the "
-                               "input to a CUDA (sm_100a) device")
+                               "input to a CUDA (sm_90a) device")
         blocks = self._blocks()
         params = []
         for blk in blocks:
@@ -388,7 +388,7 @@ class Model(nn.Module):
             return empty
         if not x.is_cuda:
             raise RuntimeError("wave_u_net_for_speech_enhancement_b200 has no CPU fallback: move the model and the "
-                               "input to a CUDA (sm_100a) device")
+                               "input to a CUDA (sm_90a) device")
         x = self._aligned(x)
         B, _, T = x.shape
         lib = _lib.load()
