@@ -129,15 +129,169 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 16] += A[64 x 16] * B[16 x 16]^T, bf16 operands, fp32 accumulators
-__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, bf16 operands, fp32 accumulators, N = 16, 32, ..., 128. The B descriptor addresses
+// N K-major rows of 128 B (8-row groups 1024 B apart). The f32 fragment is that of m64n16k16 per 16-column block, concatenated:
+// column block nb is d[8 nb .. 8 nb + 7].
+template <int N>
+__device__ __forceinline__ void wgmma_m64nNk16(float (&d)[N / 2], uint32_t a_lo, uint32_t b_lo, uint32_t hi);
+template <> __device__ __forceinline__ void wgmma_m64nNk16<16>(float (&d)[8], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
 {
     asm volatile(
         "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%8, %10};\n\tmov.b64 db, {%9, %10};\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, da, db, p, 1, 1, 0, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
         : "r"(a_lo), "r"(b_lo), "r"(hi)
         : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<32>(float (&d)[16], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%16, %18};\n\tmov.b64 db, {%17, %18};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<48>(float (&d)[24], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%24, %26};\n\tmov.b64 db, {%25, %26};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<64>(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%32, %34};\n\tmov.b64 db, {%33, %34};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<80>(float (&d)[40], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%40, %42};\n\tmov.b64 db, {%41, %42};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<96>(float (&d)[48], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%48, %50};\n\tmov.b64 db, {%49, %50};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<112>(float (&d)[56], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%56, %58};\n\tmov.b64 db, {%57, %58};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_m64nNk16<128>(float (&d)[64], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%64, %66};\n\tmov.b64 db, {%65, %66};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, da, db, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a_lo), "r"(b_lo), "r"(hi)
+        : "memory");
+}
+// NK K16 steps x MB m64 row blocks of one operand pair, each one m64n(16 NT)k16 over all of the CTA's columns, issued back to
+// back. acc[mb] is row block mb's fragment (columns past 16 NT untouched); a_lo addresses K step 0 of row block 0 (row blocks
+// are 64 rows = 512 x 16 B apart), b_lo K step 0 of the [16 NT rows x 64] weight tile; a K16 step is +32 B in both. Straight-line
+// code: ptxas serialises the wgmmas (waits for each one) when a branch it cannot prove warpgroup-uniform sits among them.
+template <int NT, int NK, int MB, int ACC>
+__device__ __forceinline__ void wgmma_batch(float (&acc)[MB][ACC], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    static_assert(8 * NT <= ACC, "accumulator fragment narrower than the MMA");
+#pragma unroll
+    for (int k = 0; k < NK; ++k)
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb)
+            wgmma_m64nNk16<16 * NT>(*reinterpret_cast<float (*)[8 * NT]>(&acc[mb][0]), a_lo + (uint32_t)(mb * 512 + 2 * k),
+                                    b_lo + (uint32_t)(2 * k), hi);
+}
+// wgmma_batch for run-time nt = columns / 16 (1 .. ACC / 8) and nk (1 .. 4): one fence, the batch, one commit (one wgmma group).
+// The dispatch branches lie outside the fence ... commit region.
+template <int MB, int ACC, int NT = ACC / 8>
+__device__ __forceinline__ void wgmma_group(int nt, int nk, float (&acc)[MB][ACC], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    if (NT == 1 || nt == NT) {
+        switch (nk) {
+        case 1: wgmma_fence(); wgmma_batch<NT, 1>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
+        case 2: wgmma_fence(); wgmma_batch<NT, 2>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
+        case 3: wgmma_fence(); wgmma_batch<NT, 3>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
+        default: wgmma_fence(); wgmma_batch<NT, 4>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
+        }
+    } else if constexpr (NT > 1) {
+        wgmma_group<MB, ACC, NT - 1>(nt, nk, acc, a_lo, b_lo, hi);
+    }
 }
 __device__ __forceinline__ void st_shared_v4_if(uint32_t addr, const uint4 &v, bool pred)
 {
@@ -484,8 +638,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     } else if (warp < kEpilogueWarps) {
         // ======================= consumer warpgroups: wgmma + epilogue =======================
         // The tile's 128 rows are split into m64 blocks over the warpgroups (large flavour: one block each, small: two); every
-        // warpgroup runs the whole K loop for its rows with the accumulators in registers (n16 column blocks), releases each
-        // operand stage once its wgmma group has completed, then applies BatchNorm + LeakyReLU straight from the fragments.
+        // warpgroup runs the whole K loop for its rows with the accumulators in registers, each MMA as wide as the CTA's
+        // columns, releases each operand stage once its wgmma groups have completed, then applies BatchNorm + LeakyReLU
+        // straight from the fragments.
         // Fragment of m64nNk16 (f32): thread (warp wq, lane) holds rows 16 wq + lane / 4 (+8) and columns 2 (lane % 4) (+1) of
         // every 8-column group.
         constexpr int NWG = kEpilogueWarps / 4;
@@ -504,15 +659,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int tile = first_tile; tile < total_tiles; tile += gridDim.x) {
             int b0, l0, n0;
             tile_coords(tile, b0, l0, n0);
-            const int Nthis = min(p.Nh, p.Npad - n0);
-            const int nblk = Nthis >> 4;
-            float acc[MB][NB][8];
+            const int nt = min(p.Nh, p.Npad - n0) >> 4;     // 16-column blocks of this CTA (the last column split may be narrower)
+            float acc[MB][8 * NB];
 #pragma unroll
             for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
-                for (int nb = 0; nb < NB; ++nb)
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) acc[mb][nb][j] = 0.f;
+                for (int j = 0; j < 8 * NB; ++j) acc[mb][j] = 0.f;
             for (int c = 0; c < p.nchunks; ++c) {
                 const ChunkInfo mci = chunk_info<UPCAT, MG, SP>(p, c);
                 const int nk = mci.nk;
@@ -529,22 +681,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     }
                     const uint32_t b_lo0 = ((b_base >> 4) & 0x3FFFu) | (1u << 16);
                     const int t0 = g * p.tg, t_end = min(KS, (g + 1) * p.tg);
-                    wgmma_fence();
+                    // one wgmma group per tap: nk K16 steps x MB row blocks, each as wide as the CTA's columns. The stage is
+                    // released once all of them have completed. (Releasing it one group late, after a wgmma.wait_group 1 behind the
+                    // next stage's first group, measured about 5 % slower end to end on an H100 at 400 W.)
 #pragma unroll 1
-                    for (int t = t0; t < t_end; ++t) {
-                        const uint32_t a_t = a_lo0 + (uint32_t)t * 8u;                 // tap shift: +128 B
-                        const uint32_t b_t = b_lo0 + (uint32_t)(t - t0) * b_step;
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            if (k >= nk) break;
-#pragma unroll
-                            for (int mb = 0; mb < MB; ++mb)
-#pragma unroll
-                                for (int nb = 0; nb < NB; ++nb)
-                                    if (nb < nblk) wgmma_n16(acc[mb][nb], a_t + (uint32_t)(mb * 512 + 2 * k), b_t + (uint32_t)(nb * 128 + 2 * k), hi);
-                        }
-                    }
-                    wgmma_commit();
+                    for (int t = t0; t < t_end; ++t)
+                        wgmma_group(nt, nk, acc, a_lo0 + (uint32_t)t * 8u,               // tap shift: +128 B
+                                    b_lo0 + (uint32_t)(t - t0) * b_step, hi);
                     wgmma_wait0();
                     if (!p.resident) {
                         if (wg_leader) mbar_arrive(b_empty + 8 * sb);
@@ -570,13 +713,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     float hsum = 0.f;
 #pragma unroll
                     for (int nb = 0; nb < NB; ++nb) {
-                        if (nb >= nblk) break;
+                        if (nb >= nt) break;
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int col = nb * 16 + 8 * e + 2 * (lane & 3);            // column inside this CTA's N range
                             const float4 s2 = *reinterpret_cast<const float4 *>(&ss[n0 + col]);
-                            const float f0 = lrelu(fmaf(acc[mb][nb][4 * e + 2 * h], s2.x, s2.y));
-                            const float f1 = lrelu(fmaf(acc[mb][nb][4 * e + 2 * h + 1], s2.z, s2.w));
+                            const float f0 = lrelu(fmaf(acc[mb][8 * nb + 4 * e + 2 * h], s2.x, s2.y));
+                            const float f1 = lrelu(fmaf(acc[mb][8 * nb + 4 * e + 2 * h + 1], s2.z, s2.w));
                             const bool col_ok = n0 + col < p.Cout;                        // Cout is even: both columns or none
                             if (p.out != nullptr && valid && col_ok) {
                                 if (SP != 0) {
@@ -1154,30 +1297,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     } else {
         // ======================= consumer warpgroups: wgmma over 64 frames each + epilogue =======================
         const int wg = warp >> 2, wq = warp & 3;
-        const int nblk = n_this >> 4;
+        const int nt = n_this >> 4;
         const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 30);
-        float acc[NB][8];
+        float acc[1][8 * NB];
 #pragma unroll
-        for (int nb = 0; nb < NB; ++nb)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[nb][j] = 0.f;
+        for (int j = 0; j < 8 * NB; ++j) acc[0][j] = 0.f;
         for (int it = 0; it < nst; ++it) {
             const uint32_t st = (uint32_t)it % (uint32_t)p.nstages, ph = ((uint32_t)it / (uint32_t)p.nstages) & 1u;
             const int kn = min(p.cps, nch - it * p.cps);
             mbar_wait(full + 8 * st, ph);
             const uint32_t a0 = (((base + st * stage_bytes) >> 4) & 0x3FFFu) | (1u << 16);
             const uint32_t w0 = (((base + st * stage_bytes + (uint32_t)p.cps * 16384u) >> 4) & 0x3FFFu) | (1u << 16);
-            wgmma_fence();
+            // one wgmma group per K chunk: 4 K16 steps, each one m64n(n_this)k16
 #pragma unroll 1
-            for (int j = 0; j < kn; ++j) {
-                const uint32_t a_lo = a0 + (uint32_t)j * 1024u + (uint32_t)wg * 512u, b_lo = w0 + (uint32_t)j * (p.w_bytes >> 4);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-#pragma unroll
-                    for (int nb = 0; nb < NB; ++nb)
-                        if (nb < nblk) wgmma_n16(acc[nb], a_lo + 2 * k, b_lo + (uint32_t)(nb * 128 + 2 * k), hi);
-            }
-            wgmma_commit();
+            for (int j = 0; j < kn; ++j)
+                wgmma_group(nt, 4, acc, a0 + (uint32_t)j * 1024u + (uint32_t)wg * 512u, w0 + (uint32_t)j * (p.w_bytes >> 4), hi);
             wgmma_wait0();
             if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * st);
         }
@@ -1186,13 +1320,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             const int b = b0 + wg * 64 + 16 * wq + (lane >> 2) + 8 * h;
 #pragma unroll
             for (int nb = 0; nb < NB; ++nb) {
-                if (nb >= nblk) break;
+                if (nb >= nt) break;
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int n = n0 + nb * 16 + 8 * e + 2 * (lane & 3);
                     const float2 s0 = __ldg(p.ss + n % p.cout), s1 = __ldg(p.ss + (n + 1) % p.cout);
-                    const uint32_t o = pack_bf16(lrelu(fmaf(acc[nb][4 * e + 2 * h], s0.x, s0.y)),
-                                                 lrelu(fmaf(acc[nb][4 * e + 2 * h + 1], s1.x, s1.y)));
+                    const uint32_t o = pack_bf16(lrelu(fmaf(acc[0][8 * nb + 4 * e + 2 * h], s0.x, s0.y)),
+                                                 lrelu(fmaf(acc[0][8 * nb + 4 * e + 2 * h + 1], s1.x, s1.y)));
                     if (b < p.B) *reinterpret_cast<uint32_t *>(p.out + (size_t)b * p.N + n) = o;
                 }
             }
