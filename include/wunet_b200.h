@@ -192,6 +192,36 @@ int wunet_train_backward_part(wunet_ctx *ctx, const float *x, const float *y, co
                               const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
                               float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                               void *stream, int part);
+/* The same three entry points with a training precision (the ones above are these with WUNET_PREC_FP32):
+ *   WUNET_PREC_FP32  fp32 FFMA in every pass;
+ *   WUNET_PREC_BF16  mixed precision: the operands of the three convolution-shaped passes — block input (after decimation, or
+ *                    interpolation + concat, computed in fp32 first), weights and dz — are rounded to bf16 and the products
+ *                    accumulated in fp32 on the wgmma tensor cores; z, BatchNorm, the head, the decimate / upsample / concat
+ *                    adjoints and all gradients stay fp32 (torch.autocast(bfloat16) semantics for Conv1d, except that z is fp32).
+ *                    The first block (Cin = 1) stays fp32. Parameters and gradients are fp32 in the reference layouts.
+ *   WUNET_PREC_FP32_TC -> WUNET_EINVAL (not a training precision).
+ * The backward must use the precision and workspace of its forward. Same call sites as above (trainer/trainer.py:35-37). */
+size_t wunet_train_workspace_bytes_prec(const wunet_ctx *ctx, int B, int T, int precision);
+int wunet_train_forward_prec(wunet_ctx *ctx, const float *x, float *y, int B, int T, const float *const *conv_w,
+                             const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                             float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                             float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision);
+int wunet_train_backward_part_prec(wunet_ctx *ctx, const float *x, const float *y, const float *dy, int B, int T,
+                                   const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                                   const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                                   float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                                   void *stream, int part, int precision);
+/* Test hook, synchronous, on caller device buffers (fp32): one convolution-shaped pass of the training step at `precision`
+ * (WUNET_PREC_FP32 or WUNET_PREC_BF16), the kernels the step itself uses. mode: 0 = direct, 1 = decimated (src0 is
+ * [B][cin0][2L], every other sample read), 2 = upsample + concat (src0 = [B][cin0][L/2] interpolated 2x linearly,
+ * align_corners=True, then src1 = [B][cin1][L]); ksize 15 with modes 0/1, 5 with mode 2 (pass 1 also takes 5 with mode 0).
+ * w = [cout][cin0 + cin1][ksize] (Conv1d, no bias).
+ *   pass 0: out[B][cout][L] = conv1d(in, w, padding = ksize/2)          (model/unet_basic.py:10,23,53)
+ *   pass 1: out[B][cin][L]  = input gradient of that conv for dz [B][cout][L]
+ *   pass 2: out[cout][cin][ksize] = weight gradient for dz [B][cout][L]
+ * No reference counterpart (autograd computes these inside loss.backward(), trainer/trainer.py:37). */
+int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, int L, int cin0, int cin1, int cout,
+                           const float *src0, const float *src1, const float *w, const float *dz, float *out);
 
 /* Introspection for tests and tuning, host-only (needs no GPU, no context): the tiling the bf16 path would use for conv
  * block `block` (1 .. 2*n_layers; block 0 = first encoder runs on CUDA cores) at batch B, frame length T, on a device with

@@ -62,6 +62,11 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_forward.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_float, vp, cs, vp]
     lib.wunet_train_backward.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, cs, vp]
     lib.wunet_train_backward_part.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, cs, vp, ci]
+    lib.wunet_train_workspace_bytes_prec.argtypes = [vp, ci, ci, ci]
+    lib.wunet_train_workspace_bytes_prec.restype = cs
+    lib.wunet_train_forward_prec.argtypes = lib.wunet_train_forward.argtypes + [ci]
+    lib.wunet_train_backward_part_prec.argtypes = lib.wunet_train_backward_part.argtypes + [ci]
+    lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     _lib = lib
     return lib
 
@@ -76,6 +81,7 @@ EXPORTED_SYMBOLS = [
     "wunet_set_weights", "wunet_workspace_bytes", "wunet_forward", "wunet_forward_host", "wunet_stream_submit", "wunet_stream_wait", "wunet_read_level",
     "wunet_last_launch_count", "wunet_profile_enable", "wunet_profile_read", "wunet_debug_plan", "wunet_debug_pair_weights",
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
+    "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]

@@ -454,10 +454,29 @@ int wunet_read_level(wunet_ctx *c, int block, const void *workspace, int B, int 
 
 int wunet_last_launch_count(const wunet_ctx *c) { return c ? c->last_launches : 0; }
 
+// training precision -> TrainPrec; -1 (with the error message set) when it is not one
+static int train_prec(int precision)
+{
+    if (precision == WUNET_PREC_FP32) return TRAIN_FP32;
+    if (precision == WUNET_PREC_BF16) return TRAIN_BF16;
+    if (precision == WUNET_PREC_FP32_TC)
+        fail(WUNET_EINVAL, "training precision WUNET_PREC_FP32_TC is not supported: use WUNET_PREC_FP32 or WUNET_PREC_BF16");
+    else
+        fail(WUNET_EINVAL, "unknown training precision %d", precision);
+    return -1;
+}
+
 size_t wunet_train_workspace_bytes(const wunet_ctx *c, int B, int T)
 {
+    return wunet_train_workspace_bytes_prec(c, B, T, WUNET_PREC_FP32);
+}
+
+size_t wunet_train_workspace_bytes_prec(const wunet_ctx *c, int B, int T, int precision)
+{
     if (check_shape(c, B, T) != WUNET_OK) return 0;
-    return train_workspace_bytes(c->n, c->ci, B, T);
+    const int prec = train_prec(precision);
+    if (prec < 0) return 0;
+    return train_workspace_bytes(c->n, c->ci, B, T, prec);
 }
 
 int wunet_train_forward(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
@@ -465,15 +484,26 @@ int wunet_train_forward(wunet_ctx *c, const float *x, float *y, int B, int T, co
                         float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
                         float momentum, void *workspace, size_t workspace_bytes, void *stream)
 {
+    return wunet_train_forward_prec(c, x, y, B, T, conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w,
+                                    out_b, momentum, workspace, workspace_bytes, stream, WUNET_PREC_FP32);
+}
+
+int wunet_train_forward_prec(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
+                             const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                             float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                             float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
+    const int prec = train_prec(precision);
+    if (prec < 0) return WUNET_EINVAL;
     if (!x || !y || !workspace || !conv_w || !conv_b || !bn_weight || !bn_bias || !bn_running_mean || !bn_running_var || !out_w || !out_b)
         return fail(WUNET_EINVAL, "null argument");
-    const size_t need = train_workspace_bytes(c->n, c->ci, B, T);
+    const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b};
-    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream)))
+    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
 }
@@ -483,8 +513,8 @@ int wunet_train_backward(wunet_ctx *c, const float *x, const float *y, const flo
                          float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight, float *const *g_bn_bias,
                          float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes, void *stream)
 {
-    return wunet_train_backward_part(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight,
-                                     g_bn_bias, g_out_w, g_out_b, workspace, workspace_bytes, stream, -1);
+    return wunet_train_backward_part_prec(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight,
+                                          g_bn_bias, g_out_w, g_out_b, workspace, workspace_bytes, stream, -1, WUNET_PREC_FP32);
 }
 
 int wunet_train_backward_part(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
@@ -493,18 +523,40 @@ int wunet_train_backward_part(wunet_ctx *c, const float *x, const float *y, cons
                               float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                               void *stream, int part)
 {
+    return wunet_train_backward_part_prec(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight,
+                                          g_bn_bias, g_out_w, g_out_b, workspace, workspace_bytes, stream, part, WUNET_PREC_FP32);
+}
+
+int wunet_train_backward_part_prec(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
+                                   const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                                   const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                                   float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                                   void *stream, int part, int precision)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
+    const int prec = train_prec(precision);
+    if (prec < 0) return WUNET_EINVAL;
     if (!x || !y || !dy || !workspace || !conv_w || !bn_weight || !bn_bias || !out_w || !g_conv_w || !g_conv_b || !g_bn_weight ||
         !g_bn_bias || !g_out_w || !g_out_b)
         return fail(WUNET_EINVAL, "null argument");
-    const size_t need = train_workspace_bytes(c->n, c->ci, B, T);
+    const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, nullptr, bn_weight, bn_bias, nullptr, nullptr, out_w, nullptr};
     const TrainGrads G{g_conv_w, g_conv_b, g_bn_weight, g_bn_bias, g_out_w, g_out_b};
-    if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part))
+    if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec))
         return fail(WUNET_ECUDA, "%s", train_error());
+    return WUNET_OK;
+}
+
+int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, int L, int cin0, int cin1, int cout,
+                           const float *src0, const float *src1, const float *w, const float *dz, float *out)
+{
+    const int prec = train_prec(precision);
+    if (prec < 0) return WUNET_EINVAL;
+    if (train_debug_conv(pass, prec, mode, ksize, B, L, cin0, cin1, cout, src0, src1, w, dz, out))
+        return fail(WUNET_EINVAL, "%s", train_error());
     return WUNET_OK;
 }
 

@@ -74,4 +74,14 @@ int launch_pack_fp32(const float *w, const float *bias, const float *g, const fl
                      const float *var, float *wp, float *scale, float *shift, int Cout, int Cin, int K,
                      cudaStream_t st);
 
+// ---- bf16 tensor-core training convolutions, implemented in wunet_train_tc.cu -----------------------
+// launch_conv_bf16: launch_conv_fp32's operator with a.wp pointing at the bf16 forward (or input-gradient) packing written by
+// train_tc_pack; ksize 15 (DIRECT, DECIM) or 5 (DIRECT, UPCAT).
+int launch_conv_bf16(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
+// dw[co][ci][k] += sum_{b,l} dz[b][co][l] * in(b, ci, l + k - pad), in read through `a` as the forward reads it (dw zeroed first)
+int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st);
+// bf16 elements of one packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout))
+size_t train_tc_packed_elems(int cout, int cin, int k);
+int train_tc_pack(const float *w, __nv_bfloat16 *wf, __nv_bfloat16 *wb, int Cout, int Cin, int K, cudaStream_t st);
+
 }  // namespace wunet

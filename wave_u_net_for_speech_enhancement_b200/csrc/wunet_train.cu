@@ -7,6 +7,8 @@
 //   weight gradient                  -> train_wgrad_kernel below (register-tiled reduction over (batch, position) tiles staged in
 //                                       shared memory, split over the batch, combined with atomicAdd).
 // The naive one-thread-per-output kernels they replace are kept as WUNET_TRAIN_NAIVE=1 (cross-check, tests).
+// TRAIN_BF16 (Model(train_precision="bf16")): the forward conv, input gradient and weight gradient of every block but the
+// first (Cin = 1) run on the bf16 tensor-core kernels of wunet_train_tc.cu instead; everything else is the same fp32 code.
 //
 // Reference: trainer/trainer.py:34-38 (forward, loss.backward()), model/unet_basic.py:77-100 with the BatchNorm1d of
 // :12, :25, :55 in .train() mode (batch statistics; running statistics updated with momentum 0.1 and the unbiased variance).
@@ -441,6 +443,19 @@ __global__ void __launch_bounds__(256) train_wgrad_kernel(const ConvArgs a, cons
         }
 }
 
+// the tiled fp32 weight gradient (dw zeroed first); mode DIRECT / DECIM: 15 taps, UPCAT: 5
+void launch_wgrad_fp32(const ConvArgs &a, const float *dz, float *dw, int mode, cudaStream_t st)
+{
+    const int lt = std::min(a.L, 128);
+    const int nco = (a.Cout + 15) / 16, nci = (a.Cin + 63) / 64;
+    const int ntiles = a.B * ((a.L + lt - 1) / lt);
+    const int slices = std::max(1, std::min(ntiles, 1184 / (nco * nci)));           // ~4 blocks per SM over the grid
+    const dim3 gt((unsigned)nco, (unsigned)nci, (unsigned)slices);
+    if (mode == SRC_DIRECT) train_wgrad_kernel<15, SRC_DIRECT><<<gt, 256, 0, st>>>(a, dz, dw, lt);
+    else if (mode == SRC_DECIM) train_wgrad_kernel<15, SRC_DECIM><<<gt, 256, 0, st>>>(a, dz, dw, lt);
+    else train_wgrad_kernel<5, SRC_UPCAT><<<gt, 256, 0, st>>>(a, dz, dw, lt);
+}
+
 struct Shape { int cin, cout, k, L, mode, cin0, cin1; };
 
 void shapes_of(int n, int ci, int T, std::vector<Shape> &sh)
@@ -459,11 +474,15 @@ struct Layout {
     std::vector<size_t> z, act, ga;      // float offsets of the pre-BN outputs, activations, activation gradients
     std::vector<size_t> mean, invstd, s1, s2;
     std::vector<size_t> wf, wb;          // the step's packed weights: forward / input-gradient operand layouts
+    std::vector<size_t> wf16, wb16;      // TRAIN_BF16 only (appended after `total` of the fp32 layout): the bf16 packings
     size_t din, ones, zeros, total;      // ones / zeros: [kMaxC] identity scale and zero shift for the linear conv epilogue
 };
 constexpr int kMaxC = 2048;
 
-void layout_of(const std::vector<Shape> &sh, int B, Layout &lo)
+// the first block (Cin = 1: a degenerate GEMM) stays on the fp32 kernels at every precision
+bool on_tc(int prec, int i) { return prec == TRAIN_BF16 && i > 0; }
+
+void layout_of(const std::vector<Shape> &sh, int B, Layout &lo, int prec = TRAIN_FP32)
 {
     const size_t nb = sh.size();
     lo.z.resize(nb); lo.act.resize(nb); lo.ga.resize(nb); lo.mean.resize(nb); lo.invstd.resize(nb); lo.s1.resize(nb); lo.s2.resize(nb); lo.wf.resize(nb); lo.wb.resize(nb);
@@ -478,6 +497,12 @@ void layout_of(const std::vector<Shape> &sh, int B, Layout &lo)
     }
     lo.din = take(din_max);
     lo.ones = take(kMaxC); lo.zeros = take(kMaxC);
+    lo.wf16.assign(nb, 0); lo.wb16.assign(nb, 0);
+    for (size_t i = 0; i < nb; ++i) {
+        if (!on_tc(prec, (int)i)) continue;
+        lo.wf16[i] = take((train_tc_packed_elems(sh[i].cout, sh[i].cin, sh[i].k) + 1) / 2);        // float units
+        lo.wb16[i] = take((train_tc_packed_elems(sh[i].cin, sh[i].cout, sh[i].k) + 1) / 2);
+    }
     lo.total = cur;
 }
 
@@ -510,24 +535,24 @@ bool train_naive()
 
 const char *train_error() { return g_train_err; }
 
-size_t train_workspace_bytes(int n, int ci, int B, int T)
+size_t train_workspace_bytes(int n, int ci, int B, int T, int prec)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
-    layout_of(sh, B, lo);
+    layout_of(sh, B, lo, prec);
     return lo.total * sizeof(float);
 }
 
 int train_forward(int n, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum, void *workspace,
-                  cudaStream_t st)
+                  cudaStream_t st, int prec)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
-    layout_of(sh, B, lo);
+    layout_of(sh, B, lo, prec);
     float *ws = static_cast<float *>(workspace);
-    const bool naive = train_naive();
+    const bool naive = train_naive() && prec == TRAIN_FP32;
     if (sh[0].cout * (2 * n) > kMaxC && !naive) return train_fail("channel plan too wide for the training kernels (%d channels)", sh[0].cout * 2 * n);
     if (!naive) {
         train_fill_kernel<<<(kMaxC + 255) / 256, 256, 0, st>>>(ws + lo.ones, 1.f, kMaxC);
@@ -538,7 +563,13 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
         ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
         float *z = ws + lo.z[i];
         const dim3 grid((unsigned)((s.L + 127) / 128), (unsigned)((s.cout + 7) / 8), (unsigned)B);
-        if (!naive) {
+        if (on_tc(prec, i)) {
+            // z = conv(bf16(in), bf16(w)) + bias on the tensor cores (fp32 accumulate); both bf16 packings for this step
+            __nv_bfloat16 *wf16 = reinterpret_cast<__nv_bfloat16 *>(ws + lo.wf16[i]), *wb16 = reinterpret_cast<__nv_bfloat16 *>(ws + lo.wb16[i]);
+            if (train_tc_pack(P.conv_w[i], wf16, wb16, s.cout, s.cin, s.k, st) < 0) return train_fail("training forward, block %d: bf16 pack failed", i);
+            a.wp = reinterpret_cast<const float *>(wf16); a.scale = ws + lo.ones; a.shift = P.conv_b[i]; a.out = z; a.linear = 1;
+            if (launch_conv_bf16(a, s.k, s.mode, st) < 0) return train_fail("training forward, block %d: bf16 conv launch failed", i);
+        } else if (!naive) {
             // z = conv(in, w) + bias through the tuned fp32 conv kernels: identity scale, shift = conv bias, no activation
             const long long nw = (long long)s.cout * s.cin * s.k;
             train_pack_kernel<<<blocks_for(nw, 256), 256, 0, st>>>(P.conv_w[i], ws + lo.wf[i], ws + lo.wb[i], s.cout, s.cin, s.k);
@@ -561,15 +592,15 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
 }
 
 int train_backward(int n, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
-                   const TrainGrads &G, void *workspace, cudaStream_t st, int part)
+                   const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
-    layout_of(sh, B, lo);
+    layout_of(sh, B, lo, prec);
     float *ws = static_cast<float *>(workspace);
     const int last = 2 * n, C = sh[last].cout;
-    const bool naive = train_naive();
+    const bool naive = train_naive() && prec == TRAIN_FP32;
     if (part < -1 || part > 1) return train_fail("training backward: part must be -1, 0 or 1 (got %d)", part);
     if (part != 1) {
         cudaMemsetAsync(G.out_w, 0, (C + 1) * sizeof(float), st);
@@ -592,15 +623,10 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         const ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
         cudaMemsetAsync(G.conv_w[i], 0, (size_t)s.cout * s.cin * s.k * sizeof(float), st);
         const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
-        if (!naive) {
-            const int lt = std::min(s.L, 128);
-            const int nco = (s.cout + 15) / 16, nci = (s.cin + 63) / 64;
-            const int ntiles = B * ((s.L + lt - 1) / lt);
-            const int slices = std::max(1, std::min(ntiles, 1184 / (nco * nci)));           // ~4 blocks per SM over the grid
-            const dim3 gt((unsigned)nco, (unsigned)nci, (unsigned)slices);
-            if (s.mode == SRC_DIRECT) train_wgrad_kernel<15, SRC_DIRECT><<<gt, 256, 0, st>>>(a, ga, G.conv_w[i], lt);
-            else if (s.mode == SRC_DECIM) train_wgrad_kernel<15, SRC_DECIM><<<gt, 256, 0, st>>>(a, ga, G.conv_w[i], lt);
-            else train_wgrad_kernel<5, SRC_UPCAT><<<gt, 256, 0, st>>>(a, ga, G.conv_w[i], lt);
+        if (on_tc(prec, i)) {
+            if (launch_wgrad_bf16(a, ga, G.conv_w[i], s.k, s.mode, st) < 0) return train_fail("training backward, block %d: bf16 weight-gradient launch failed", i);
+        } else if (!naive) {
+            launch_wgrad_fp32(a, ga, G.conv_w[i], s.mode, st);
         } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
         else if (s.mode == SRC_DECIM) train_conv_bwd_weight_kernel<15, SRC_DECIM><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
         else train_conv_bwd_weight_kernel<5, SRC_UPCAT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
@@ -613,7 +639,10 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
                 ConvArgs d{};
                 d.src0 = ga; d.wp = ws + lo.wb[i]; d.scale = ws + lo.ones; d.shift = ws + lo.zeros; d.out = din;
                 d.B = B; d.L = s.L; d.Cin = s.cout; d.Cin0 = s.cout; d.Cin1 = 0; d.Cout = s.cin; d.linear = 1;
-                if (launch_conv_fp32(d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: input-gradient conv launch failed", i);
+                if (on_tc(prec, i)) {
+                    d.wp = ws + lo.wb16[i];                    // the bf16 packing the forward wrote
+                    if (launch_conv_bf16(d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: bf16 input-gradient launch failed", i);
+                } else if (launch_conv_fp32(d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: input-gradient conv launch failed", i);
             } else if (s.k == 15) train_conv_bwd_data_kernel<15><<<gd, 128, 0, st>>>(ga, P.conv_w[i], din, B, s.cin, s.cout, s.L);
             else train_conv_bwd_data_kernel<5><<<gd, 128, 0, st>>>(ga, P.conv_w[i], din, B, s.cin, s.cout, s.L);
             if (s.mode == SRC_DECIM) {
@@ -629,6 +658,55 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return train_fail("training backward, block %d: %s", i, cudaGetErrorString(e));
     }
+    return 0;
+}
+
+int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int Cin0, int Cin1, int Cout, const float *src0,
+                     const float *src1, const float *w, const float *dz, float *out)
+{
+    const bool ok_mode = (ksize == 15 && (mode == SRC_DIRECT || mode == SRC_DECIM)) || (ksize == 5 && mode == SRC_UPCAT) ||
+                         (ksize == 5 && mode == SRC_DIRECT && pass == 1);
+    if (pass < 0 || pass > 2 || (prec != TRAIN_FP32 && prec != TRAIN_BF16) || !ok_mode || B < 1 || L < 1 || Cin0 < 1 ||
+        Cin1 < 0 || Cout < 1 || (mode != SRC_UPCAT && Cin1 != 0) || (mode == SRC_UPCAT && (L < 2 || L % 2 != 0 || Cin1 < 1)) ||
+        !w || !out || (pass != 1 && !src0) || (pass != 1 && mode == SRC_UPCAT && !src1) || (pass != 0 && !dz))
+        return train_fail("debug conv: bad arguments");
+    const int Cin = Cin0 + Cin1, K = ksize, cmax = std::max(Cin, Cout);
+    ConvArgs a{};
+    a.src0 = src0; a.src1 = src1; a.B = B; a.L = L; a.Cin = Cin; a.Cin0 = mode == SRC_UPCAT ? Cin0 : Cin; a.Cin1 = Cin1; a.Cout = Cout;
+    a.up_scale = (mode == SRC_UPCAT && L > 1) ? (float)(L / 2 - 1) / (float)(L - 1) : 0.f;
+    float *buf = nullptr;
+    const size_t nw = (size_t)Cout * Cin * K, cpad = (cmax + 63) / 64 * 64, wpad = (nw + 63) / 64 * 64;      // 256-byte aligned parts
+    const size_t n16 = train_tc_packed_elems(Cout, Cin, K) + train_tc_packed_elems(Cin, Cout, K);
+    if (cudaMalloc(&buf, (2 * cpad + 2 * wpad + (n16 + 1) / 2) * sizeof(float)) != cudaSuccess)
+        return train_fail("debug conv: %s", cudaGetErrorString(cudaGetLastError()));
+    float *ones = buf, *zeros = buf + cpad, *wf = zeros + cpad, *wb = wf + wpad;
+    __nv_bfloat16 *wf16 = reinterpret_cast<__nv_bfloat16 *>(wb + wpad), *wb16 = wf16 + train_tc_packed_elems(Cout, Cin, K);
+    const cudaStream_t st = 0;
+    train_fill_kernel<<<(cmax + 255) / 256, 256, 0, st>>>(ones, 1.f, cmax);
+    train_fill_kernel<<<(cmax + 255) / 256, 256, 0, st>>>(zeros, 0.f, cmax);
+    const bool tc = prec == TRAIN_BF16;
+    int rc = 0;
+    if (pass == 2) {
+        cudaMemsetAsync(out, 0, nw * sizeof(float), st);
+        if (tc) rc = launch_wgrad_bf16(a, dz, out, K, mode, st);
+        else launch_wgrad_fp32(a, dz, out, mode, st);
+    } else {
+        if (tc) rc = train_tc_pack(w, wf16, wb16, Cout, Cin, K, st);
+        else train_pack_kernel<<<blocks_for((long long)nw, 256), 256, 0, st>>>(w, wf, wb, Cout, Cin, K);
+        if (pass == 0) {
+            a.wp = tc ? reinterpret_cast<const float *>(wf16) : wf; a.scale = ones; a.shift = zeros; a.out = out; a.linear = 1;
+            if (rc >= 0) rc = tc ? launch_conv_bf16(a, K, mode, st) : launch_conv_fp32(a, K, mode, st);
+        } else {
+            ConvArgs d{};
+            d.src0 = dz; d.wp = tc ? reinterpret_cast<const float *>(wb16) : wb; d.scale = ones; d.shift = zeros; d.out = out;
+            d.B = B; d.L = L; d.Cin = Cout; d.Cin0 = Cout; d.Cin1 = 0; d.Cout = Cin; d.linear = 1;
+            if (rc >= 0) rc = tc ? launch_conv_bf16(d, K, SRC_DIRECT, st) : launch_conv_fp32(d, K, SRC_DIRECT, st);
+        }
+    }
+    const cudaError_t e = cudaDeviceSynchronize();
+    cudaFree(buf);
+    if (rc < 0) return train_fail("debug conv: launch failed");
+    if (e != cudaSuccess) return train_fail("debug conv: %s", cudaGetErrorString(e));
     return 0;
 }
 

@@ -22,15 +22,25 @@ struct TrainGrads {
     float *out_w, *out_b;
 };
 
+// Arithmetic of the three convolution-shaped passes. TRAIN_FP32: fp32 FFMA. TRAIN_BF16: bf16 operands (block input, weights,
+// dz; round to nearest), fp32 accumulation on the tensor cores (wunet_train_tc.cu); the first block stays fp32. Everything else
+// is fp32 at both precisions. The workspace of TRAIN_BF16 is the fp32 one plus the bf16 weight packings.
+enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1 };
+
 const char *train_error();
-size_t train_workspace_bytes(int n_layers, int ci, int B, int T);
+size_t train_workspace_bytes(int n_layers, int ci, int B, int T, int prec = TRAIN_FP32);
 // y = model(x) with BatchNorm in training mode; keeps every pre-BN output and activation in `workspace` for the backward
 int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum,
-                  void *workspace, cudaStream_t stream);
+                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32);
 // gradients of every parameter for the upstream gradient dy of the output; `workspace` as left by train_forward.
 // part: -1 = the whole backward; 0 = head + decoder blocks (their gradients are complete afterwards: a data-parallel caller
 // starts reducing them while part 1 runs); 1 = middle + encoder blocks (must follow part 0 on the same stream).
 int train_backward(int n_layers, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
-                   const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1);
+                   const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1, int prec = TRAIN_FP32);
+// One convolution-shaped pass on caller device buffers (test hook): pass 0 = forward conv out[B][Cout][L] = conv(in, w);
+// 1 = input gradient out[B][Cin][L] of dz [B][Cout][L] (Conv1d padding, no mode); 2 = weight gradient out[Cout][Cin][K] =
+// sum dz * in. `in` is built from src0 / src1 per `mode` as in the forward (ConvArgs). Synchronous.
+int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int Cin0, int Cin1, int Cout, const float *src0,
+                     const float *src1, const float *w, const float *dz, float *out);
 
 }  // namespace wunet

@@ -147,7 +147,8 @@ class _NativeTrainStep(torch.autograd.Function):
         B, _, T = x.shape
         with torch.cuda.device(x.device):
             c = model._context(x.device)
-            nbytes = lib.wunet_train_workspace_bytes(c, B, T)
+            prec = _lib.PRECISIONS[model.train_precision]
+            nbytes = lib.wunet_train_workspace_bytes_prec(c, B, T, prec)
             if nbytes == 0:
                 _lib.check(-1)
             ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
@@ -161,10 +162,11 @@ class _NativeTrainStep(torch.autograd.Function):
             momentum = float(blocks[0][1].momentum)
             stream = torch.cuda.current_stream(x.device).cuda_stream
             P = _NativeTrainStep._ptr_array
-            _lib.check(lib.wunet_train_forward(c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b),
-                                               P(rmean), P(rvar), params[-2].data_ptr(), params[-1].data_ptr(), momentum,
-                                               ws.data_ptr(), ws.numel(), stream))
-        ctx.model, ctx.ws, ctx.nb = model, ws, nb
+            _lib.check(lib.wunet_train_forward_prec(c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b),
+                                                    P(rmean), P(rvar), params[-2].data_ptr(), params[-1].data_ptr(), momentum,
+                                                    ws.data_ptr(), ws.numel(), stream, prec))
+        # the backward runs at the precision of ITS forward (and reads the bf16 weight packings that forward left in ws)
+        ctx.model, ctx.ws, ctx.nb, ctx.prec = model, ws, nb, prec
         ctx.save_for_backward(x, y, *params)
         return y
 
@@ -187,11 +189,11 @@ class _NativeTrainStep(torch.autograd.Function):
             P = _NativeTrainStep._ptr_array
             sel = lambda ts, k: [ts[4 * i + k] for i in range(nb)]          # noqa: E731
             for part in ((0, 1) if reduce else (-1,)):
-                _lib.check(lib.wunet_train_backward_part(c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)),
-                                                         P(sel(params, 2)), P(sel(params, 3)), params[-2].data_ptr(),
-                                                         P(sel(grads, 0)), P(sel(grads, 1)), P(sel(grads, 2)), P(sel(grads, 3)),
-                                                         grads[-2].data_ptr(), grads[-1].data_ptr(), ctx.ws.data_ptr(),
-                                                         ctx.ws.numel(), stream, part))
+                _lib.check(lib.wunet_train_backward_part_prec(c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)),
+                                                              P(sel(params, 2)), P(sel(params, 3)), params[-2].data_ptr(),
+                                                              P(sel(grads, 0)), P(sel(grads, 1)), P(sel(grads, 2)), P(sel(grads, 3)),
+                                                              grads[-2].data_ptr(), grads[-1].data_ptr(), ctx.ws.data_ptr(),
+                                                              ctx.ws.numel(), stream, part, ctx.prec))
                 if reduce:
                     # head + decoder gradients are final after part 0: their all-reduce overlaps part 1 (middle + encoders)
                     bucket.reduce_part(part)
@@ -220,10 +222,16 @@ class Model(nn.Module):
     data_parallel  "auto" (default): when ``torch.distributed`` is initialised with more than one rank (one process per
                    GPU, SURVEY §8e) the native backward averages the gradients over the ranks — one flat bucket,
                    all-reduced in two parts so that the first overlaps the rest of the backward. "off": never.
+    train_precision  arithmetic of the native training step's three convolution-shaped passes (forward conv, input
+                   gradient, weight gradient). "fp32" (default): fp32 FFMA. "bf16": mixed precision — their operands (block
+                   input, weights, dz) are rounded to bf16 and the products accumulated in fp32 on the tensor cores; z,
+                   BatchNorm, the head and all gradients stay fp32, parameters stay fp32 (the caller's optimizer is unchanged).
+                   ``torch.autocast(bfloat16)`` semantics for Conv1d, except that z is kept in fp32. Only with
+                   train_backend="native". Not part of the state_dict.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
-                 train_backend: str = "native", data_parallel: str = "auto"):
+                 train_backend: str = "native", data_parallel: str = "auto", train_precision: str = "fp32"):
         super().__init__()
         if precision not in _lib.PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(_lib.PRECISIONS)}, got {precision!r}")
@@ -233,9 +241,14 @@ class Model(nn.Module):
         self.channels_interval = channels_interval
         if data_parallel not in ("auto", "off"):
             raise ValueError("data_parallel must be 'auto' or 'off'")
+        if train_precision not in ("fp32", "bf16"):
+            raise ValueError(f"train_precision must be 'fp32' or 'bf16', got {train_precision!r}")
+        if train_precision != "fp32" and train_backend != "native":
+            raise ValueError(f"train_precision={train_precision!r} needs train_backend='native' (got {train_backend!r})")
         self.precision = precision
         self.train_backend = train_backend
         self.data_parallel = data_parallel
+        self.train_precision = train_precision
         n, ci = n_layers, channels_interval
 
         enc_in = [1] + [i * ci for i in range(1, n)]
@@ -336,8 +349,8 @@ class Model(nn.Module):
     def _forward_train_native(self, x: torch.Tensor) -> torch.Tensor:
         """Training-mode forward through libwunet_b200 (wunet_train_forward / wunet_train_backward behind a
         torch.autograd.Function): BatchNorm uses batch statistics and updates its running buffers, ``loss.backward()`` fills
-        ``.grad`` of all 102 parameters, the caller's optimizer is used unchanged (trainer/trainer.py:34-38). fp32,
-        correctness-first kernels (SURVEY §8f row N1)."""
+        ``.grad`` of all 102 parameters, the caller's optimizer is used unchanged (trainer/trainer.py:34-38). fp32 or, with
+        ``train_precision="bf16"``, bf16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
         if not x.is_cuda:
             raise RuntimeError("wave_u_net_for_speech_enhancement_b200 has no CPU fallback: move the model and the "
