@@ -233,6 +233,10 @@ int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, 
  *  [23] TMA bytes per input chunk  [24] input rows used  [25] unused (0)  [26] dynamic shared memory bytes
  *  [27] threads per CTA  [28] CTAs per SM  [29] grid  [30] small (two-CTAs-per-SM) flavour  [31] tiles per frame */
 int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity);
+/* The same query for a tensor-core precision: WUNET_PREC_BF16 (= wunet_debug_plan) or WUNET_PREC_FP32_TC (the split-precision
+ * plan: no row-pair form, no dense GEMM, block 0 on CUDA cores). WUNET_PREC_FP32 -> WUNET_EINVAL. */
+int wunet_debug_plan_prec(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
+                          int precision);
 
 /* Introspection for tests, host-only: the "row-pair" form of one conv block's weights (WUNET_TC_PAIR, DESIGN.md 5.1). A block
  * with `ksize` taps over positions (w = [cout][cin0 + cin1][ksize] fp32, reference layout; model/unet_basic.py:10,23) is the same

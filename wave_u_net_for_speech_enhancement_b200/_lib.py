@@ -56,6 +56,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_profile_enable.argtypes = [vp, ci]
     lib.wunet_profile_read.argtypes = [vp, vp, ci, ctypes.POINTER(ci)]
     lib.wunet_debug_plan.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ci), ci]
+    lib.wunet_debug_plan_prec.argtypes = lib.wunet_debug_plan.argtypes + [ci]
     lib.wunet_debug_pair_weights.argtypes = [vp, ci, ci, ci, ci, ci, vp]
     lib.wunet_train_workspace_bytes.argtypes = [vp, ci, ci]
     lib.wunet_train_workspace_bytes.restype = cs
@@ -79,7 +80,8 @@ def check(rc: int) -> None:
 EXPORTED_SYMBOLS = [
     "wunet_version", "wunet_last_error", "wunet_create", "wunet_destroy", "wunet_num_blocks", "wunet_block_shape",
     "wunet_set_weights", "wunet_workspace_bytes", "wunet_forward", "wunet_forward_host", "wunet_stream_submit", "wunet_stream_wait", "wunet_read_level",
-    "wunet_last_launch_count", "wunet_profile_enable", "wunet_profile_read", "wunet_debug_plan", "wunet_debug_pair_weights",
+    "wunet_last_launch_count", "wunet_profile_enable", "wunet_profile_read", "wunet_debug_plan", "wunet_debug_plan_prec",
+    "wunet_debug_pair_weights",
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
@@ -91,8 +93,9 @@ PLAN_FIELDS = ["L", "Cin0", "Cin1", "Cout", "Npad", "Nh", "nsplit", "Nstride", "
                "rows_used", "tmem_cols", "smem", "threads", "per_sm", "grid", "small", "tiles_per_frame"]
 
 
-def debug_plan(n_layers: int, channels_interval: int, B: int, T: int, block: int, num_sms: int = 148) -> dict:
-    """The tiling the bf16 path would choose for one conv block (host-only query: works without a GPU)."""
+def debug_plan(n_layers: int, channels_interval: int, B: int, T: int, block: int, num_sms: int = 148,
+               precision: str = "bf16") -> dict:
+    """The tiling the bf16 (or fp32_tc) path would choose for one conv block (host-only query: works without a GPU)."""
     buf = (ctypes.c_int * 32)()
-    check(load().wunet_debug_plan(n_layers, channels_interval, B, T, block, num_sms, buf, 32))
+    check(load().wunet_debug_plan_prec(n_layers, channels_interval, B, T, block, num_sms, buf, 32, PRECISIONS[precision]))
     return dict(zip(PLAN_FIELDS, [int(v) for v in buf]))

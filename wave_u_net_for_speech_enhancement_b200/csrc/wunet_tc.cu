@@ -1709,7 +1709,8 @@ struct TcState {
     TcLevel pair_lv[2];                // [0] block 1, [1] block 2n (cin0 / cin1 / cout = virtual counts, k = pair taps)
     float *pair_w[2] = {nullptr, nullptr}, *pair_scale[2] = {nullptr, nullptr}, *pair_shift[2] = {nullptr, nullptr};
     bool pair_ok[2] = {false, false};
-    int num_sms = 148;
+    int num_sms = 148;                 // SM count the plan and the persistent grids are sized for (WUNET_TC_SMS, else dev_sms)
+    int dev_sms = 148;                 // the device's multiprocessor count
     cudaStream_t copy_in = nullptr, copy_out = nullptr;     // host pipeline: H2D / D2H streams
     cudaEvent_t ev_in[8] = {}, ev_out[8] = {};
     long long *trace = nullptr;        // development: WUNET_TC_TRACE builds + WUNET_TC_TRACE_LEVEL=<block>
@@ -1720,6 +1721,7 @@ struct TcState {
     const float *plan_x = nullptr;
     float *plan_y = nullptr;
     std::string plan_ovr;              // WUNET_TC_OVR value the cached plan was built with
+    int plan_sms = 0;                  // num_sms the cached plan was built with
     int plan_mode = 0;                 // 0: bf16 plan, 1: split-precision (fp32_tc) plan
     TcPlan plan;
 };
@@ -2339,10 +2341,10 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
     return 0;
 }
 
-int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *f, int cap)
+int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *f, int cap, int mode)
 {
     const char *e0 = getenv("WUNET_TC_ENC0");
-    const bool g8 = block == 0 && e0 && e0[0] == '1';        // block 0 has a tensor-core plan only in its group-of-8 form
+    const bool g8 = !mode && block == 0 && e0 && e0[0] == '1';    // block 0 has a tensor-core plan only in its group-of-8 form (bf16)
     if (nblocks != 2 * n + 1 || (block < 1 && !g8) || block >= nblocks) return tc_fail("block %d out of range (1..%d)", block, 2 * n);
     if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
     if (cap < 32 || !f) return tc_fail("need room for 32 fields");
@@ -2369,7 +2371,11 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
     const std::string ovr_s = ovr ? ovr : "";
     const char *ge = getenv("WUNET_TC_GEMM");
     bool planned = false;
-    {
+    if (mode) {
+        // split precision (fp32_tc): every block on conv_tc_kernel in split form, no row-pair form, no dense GEMM (build_plan)
+        if (plan_block(levels[block], block, n, B, T, num_sms, ovr_s, P, true, 0)) return -1;
+        planned = true;
+    } else {
         // row-pair mode of block 1 (WUNET_TC_PAIR bit 0), planned like build_plan does
         const char *pe = getenv("WUNET_TC_PAIR");
         const int pmask = pe ? atoi(pe) & 1 : 1;
@@ -2425,14 +2431,23 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
         cudaFuncSetAttribute(enc0_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         int dev = 0, sms = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
-            st->num_sms = sms;
+            st->dev_sms = sms;
         st->attr_set = true;
     }
     (void)x; (void)y;
+    // WUNET_TC_SMS=<n> (test hook): plan and size the persistent grids as on a device with n SMs. A grid smaller than the device
+    // is always legal, so one GPU can run the plan of any other SM count (n = 1: one CTA, two in the small flavour, per block).
+    int sms = st->dev_sms;
+    if (const char *se = getenv("WUNET_TC_SMS")) {
+        sms = atoi(se);
+        if (sms < 1) return tc_fail("WUNET_TC_SMS must be a positive SM count (got \"%s\")", se);
+    }
+    st->num_sms = sms;
     const char *ovr = getenv("WUNET_TC_OVR");
     const std::string ovr_s = ovr ? ovr : "";
-    if (st->plan_ws != ws || st->plan_B != B || st->plan_T != T || st->plan_ovr != ovr_s || st->plan_mode != mode) {
+    if (st->plan_ws != ws || st->plan_B != B || st->plan_T != T || st->plan_ovr != ovr_s || st->plan_sms != sms || st->plan_mode != mode) {
         st->plan_ovr = ovr_s;
+        st->plan_sms = sms;
         st->plan_ws = nullptr;
         if (build_plan(st, nullptr, nullptr, B, T, ws, mode, stream)) return -1;
     }

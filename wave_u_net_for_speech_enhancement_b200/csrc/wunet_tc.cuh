@@ -29,9 +29,10 @@ int tc_forward_host(TcState *st, const float *x_host, float *y_host, float *x_de
                     cudaStream_t stream, int *launches, int mode = 0);
 int tc_read_level(TcState *st, int block, const void *ws, int B, int T, float *out_ncl, cudaStream_t stream, int mode = 0);
 void tc_destroy(TcState *st);
-// host-only: the tiling build_plan would choose for `block` (32 ints, see wunet_debug_plan in include/wunet_b200.h)
+// host-only: the tiling build_plan would choose for `block` (32 ints, see wunet_debug_plan in include/wunet_b200.h); mode 1 =
+// the split-precision (fp32_tc) plan
 int tc_debug_plan(int n_layers, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *fields,
-                  int capacity);
+                  int capacity, int mode = 0);
 
 // host-only: row-pair expansion of [Cout][C0+C1][K] weights to [2 Cout][2 (C0+C1)][K'] (tests of the WUNET_TC_PAIR packing)
 int tc_debug_pair_weights(const float *w, int Cout, int C0, int C1, int K, int dec, float *out);
