@@ -211,6 +211,30 @@ int wunet_train_backward_part_prec(wunet_ctx *ctx, const float *x, const float *
                                    const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
                                    float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                                    void *stream, int part, int precision);
+
+/* The training step with flags and the input gradient (the _prec entry points above are these with flags = 0, dx = NULL).
+ * Serves autograd through the model beyond a plain training step: x.grad for whatever sits upstream of the model (a cascade,
+ * a learnable front end, an adversarial perturbation), and eval-mode BatchNorm for fine-tuning with frozen statistics. */
+#define WUNET_TRAIN_FROZEN_BN      1  /* BatchNorm uses (and never updates) the running statistics: eval-mode BN */
+#define WUNET_TRAIN_NO_PARAM_GRADS 2  /* backward: no parameter gradients (g_* may be NULL), only dx */
+/* wunet_train_forward_ex: with WUNET_TRAIN_FROZEN_BN, BatchNorm normalises by bn_running_mean / bn_running_var, which are only
+ *   read (momentum is unused): model/unet_basic.py in .eval() mode, with the activations kept for the backward. The forward
+ *   ignores WUNET_TRAIN_NO_PARAM_GRADS. The workspace size is wunet_train_workspace_bytes_prec (frozen mode needs nothing extra).
+ * wunet_train_backward_ex: dx [B][1][T] (device, or NULL) is fully overwritten with the gradient of x. It belongs to part 1
+ *   (block 0 is there): pass it with part -1 or 1; dx with part 0 is WUNET_EINVAL. With WUNET_TRAIN_NO_PARAM_GRADS no weight
+ *   gradient, bias or BatchNorm-parameter reduction runs and nothing is written through g_*.
+ * The backward must use the precision, the workspace and the WUNET_TRAIN_FROZEN_BN bit of its forward.
+ * Unknown flag bits -> WUNET_EINVAL. Call sites: loss.backward() through model(x) with x.requires_grad in .train() mode, and
+ * through model(x) in .eval() mode (trainer/trainer.py:35-37 with model.eval()). */
+int wunet_train_forward_ex(wunet_ctx *ctx, const float *x, float *y, int B, int T, const float *const *conv_w,
+                           const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                           float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                           float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags);
+int wunet_train_backward_ex(wunet_ctx *ctx, const float *x, const float *y, const float *dy, int B, int T,
+                            const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                            const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                            float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                            void *stream, float *dx, int part, int precision, int flags);
 /* Test hook, synchronous, on caller device buffers (fp32): one convolution-shaped pass of the training step at `precision`
  * (WUNET_PREC_FP32 or WUNET_PREC_BF16), the kernels the step itself uses. mode: 0 = direct, 1 = decimated (src0 is
  * [B][cin0][2L], every other sample read), 2 = upsample + concat (src0 = [B][cin0][L/2] interpolated 2x linearly,

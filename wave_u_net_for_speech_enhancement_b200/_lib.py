@@ -12,6 +12,9 @@ PREC_BF16 = 1
 PREC_FP32_TC = 2
 PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC}
 
+TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mode BatchNorm
+TRAIN_NO_PARAM_GRADS = 2   # backward: input gradient only
+
 _lib = None
 
 
@@ -67,6 +70,8 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_workspace_bytes_prec.restype = cs
     lib.wunet_train_forward_prec.argtypes = lib.wunet_train_forward.argtypes + [ci]
     lib.wunet_train_backward_part_prec.argtypes = lib.wunet_train_backward_part.argtypes + [ci]
+    lib.wunet_train_forward_ex.argtypes = lib.wunet_train_forward_prec.argtypes + [ci]
+    lib.wunet_train_backward_ex.argtypes = lib.wunet_train_backward.argtypes + [vp, ci, ci, ci]
     lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     _lib = lib
     return lib
@@ -84,6 +89,7 @@ EXPORTED_SYMBOLS = [
     "wunet_debug_pair_weights",
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
+    "wunet_train_forward_ex", "wunet_train_backward_ex",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]

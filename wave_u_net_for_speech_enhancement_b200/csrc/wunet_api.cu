@@ -493,17 +493,30 @@ int wunet_train_forward_prec(wunet_ctx *c, const float *x, float *y, int B, int 
                              float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
                              float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision)
 {
+    return wunet_train_forward_ex(c, x, y, B, T, conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w,
+                                  out_b, momentum, workspace, workspace_bytes, stream, precision, 0);
+}
+
+static const int kTrainFlags = WUNET_TRAIN_FROZEN_BN | WUNET_TRAIN_NO_PARAM_GRADS;
+
+int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
+                           const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                           float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                           float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
     const int prec = train_prec(precision);
     if (prec < 0) return WUNET_EINVAL;
+    if (flags & ~kTrainFlags) return fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
     if (!x || !y || !workspace || !conv_w || !conv_b || !bn_weight || !bn_bias || !bn_running_mean || !bn_running_var || !out_w || !out_b)
         return fail(WUNET_EINVAL, "null argument");
     const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b};
-    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec))
+    const int tflags = (flags & WUNET_TRAIN_FROZEN_BN) ? TRAIN_FROZEN_BN : 0;        // NO_PARAM_GRADS: nothing to do here
+    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec, tflags))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
 }
@@ -533,19 +546,33 @@ int wunet_train_backward_part_prec(wunet_ctx *c, const float *x, const float *y,
                                    float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                                    void *stream, int part, int precision)
 {
+    return wunet_train_backward_ex(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight, g_bn_bias,
+                                   g_out_w, g_out_b, workspace, workspace_bytes, stream, nullptr, part, precision, 0);
+}
+
+int wunet_train_backward_ex(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
+                            const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                            const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                            float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                            void *stream, float *dx, int part, int precision, int flags)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
     const int prec = train_prec(precision);
     if (prec < 0) return WUNET_EINVAL;
-    if (!x || !y || !dy || !workspace || !conv_w || !bn_weight || !bn_bias || !out_w || !g_conv_w || !g_conv_b || !g_bn_weight ||
-        !g_bn_bias || !g_out_w || !g_out_b)
+    if (flags & ~kTrainFlags) return fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
+    if (dx && part == 0) return fail(WUNET_EINVAL, "dx belongs to part 1 (block 0): pass it with part -1 or 1, not 0");
+    const bool pgrads = !(flags & WUNET_TRAIN_NO_PARAM_GRADS);
+    if (!x || !y || !dy || !workspace || !conv_w || !bn_weight || !bn_bias || !out_w ||
+        (pgrads && (!g_conv_w || !g_conv_b || !g_bn_weight || !g_bn_bias || !g_out_w || !g_out_b)))
         return fail(WUNET_EINVAL, "null argument");
     const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, nullptr, bn_weight, bn_bias, nullptr, nullptr, out_w, nullptr};
     const TrainGrads G{g_conv_w, g_conv_b, g_bn_weight, g_bn_bias, g_out_w, g_out_b};
-    if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec))
+    const int tflags = ((flags & WUNET_TRAIN_FROZEN_BN) ? TRAIN_FROZEN_BN : 0) | (pgrads ? 0 : TRAIN_NO_PARAM_GRADS);
+    if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec, dx, tflags))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
 }

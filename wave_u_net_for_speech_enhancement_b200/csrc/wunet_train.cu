@@ -9,6 +9,9 @@
 // The naive one-thread-per-output kernels they replace are kept as WUNET_TRAIN_NAIVE=1 (cross-check, tests).
 // TRAIN_BF16 (Model(train_precision="bf16")): the forward conv, input gradient and weight gradient of every block but the
 // first (Cin = 1) run on the bf16 tensor-core kernels of wunet_train_tc.cu instead; everything else is the same fp32 code.
+// TRAIN_FROZEN_BN (eval-mode BatchNorm: running statistics, never updated) and TRAIN_NO_PARAM_GRADS (input gradient only) only
+// change the BatchNorm arithmetic and which reductions run; the convolution-shaped passes are the same kernels. The input
+// gradient dx is train_input_grad_kernel below (head's raw-input channel + block 0's transposed conv).
 //
 // Reference: trainer/trainer.py:34-38 (forward, loss.backward()), model/unet_basic.py:77-100 with the BatchNorm1d of
 // :12, :25, :55 in .train() mode (batch statistics; running statistics updated with momentum 0.1 and the unbiased variance).
@@ -116,6 +119,17 @@ __global__ void __launch_bounds__(256) train_bn_stats_kernel(const float *__rest
     }
 }
 
+// eval-mode BatchNorm (TRAIN_FROZEN_BN, model/unet_basic.py in .eval()): normalise by the running statistics, rounding invstd
+// as the batch-statistics path does; the running buffers are only read
+__global__ void train_bn_frozen_stats_kernel(const float *__restrict__ running_mean, const float *__restrict__ running_var,
+                                             float *__restrict__ mean, float *__restrict__ invstd, int C)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    mean[c] = running_mean[c];
+    invstd[c] = (float)(1.0 / sqrt((double)running_var[c] + (double)kBnEps));
+}
+
 // a = LeakyReLU(gamma * (z - mean) * invstd + beta)
 __global__ void train_bn_act_kernel(const float *__restrict__ z, const float *__restrict__ mean, const float *__restrict__ invstd,
                                     const float *__restrict__ gamma, const float *__restrict__ beta, float *__restrict__ act,
@@ -133,6 +147,7 @@ __global__ void train_bn_act_kernel(const float *__restrict__ z, const float *__
 // ---------------------------------------------------------------------------------------------
 // head: y = tanh(sum_c Wo[c] cat[c] + bo), cat = [a_last (C channels) | x]   (model/unet_basic.py:98-99)
 //   dpre = dy (1 - y^2);  dWo[c] = sum dpre cat[c];  dbo = sum dpre;  d a_last[c] = Wo[c] dpre
+// g_wo == nullptr (TRAIN_NO_PARAM_GRADS): d a_last only
 __global__ void __launch_bounds__(256) train_head_bwd_kernel(const float *__restrict__ dy, const float *__restrict__ y,
                                                              const float *__restrict__ a_last, const float *__restrict__ x,
                                                              const float *__restrict__ wo, float *__restrict__ ga_last,
@@ -143,6 +158,11 @@ __global__ void __launch_bounds__(256) train_head_bwd_kernel(const float *__rest
     const int b = ok ? (int)(i / T) : 0, l = ok ? (int)(i - (long long)b * T) : 0;
     const float yv = ok ? y[i] : 0.f;
     const float dpre = ok ? dy[i] * (1.f - yv * yv) : 0.f;
+    if (!g_wo) {
+        if (ok)
+            for (int c = 0; c < C; ++c) ga_last[((size_t)b * C + c) * T + l] = wo[c] * dpre;
+        return;
+    }
     for (int c = 0; c <= C; ++c) {
         float v;
         if (c < C) {
@@ -185,14 +205,15 @@ __global__ void __launch_bounds__(256) train_bn_bwd_stats_kernel(const float *__
     const double t1 = block_sum(a1, sh);
     const double t2 = block_sum(a2, sh);
     if (threadIdx.x == 0) {
-        g_beta[c] = (float)t1;
-        g_gamma[c] = (float)t2;
+        if (g_beta) g_beta[c] = (float)t1;                     // null under TRAIN_NO_PARAM_GRADS
+        if (g_gamma) g_gamma[c] = (float)t2;
         s1[c] = (float)(t1 / (double)n);                        // mean(dy), mean(dy zh): what the input gradient needs
         s2[c] = (float)(t2 / (double)n);
     }
 }
 
 //   dz = invstd gamma (dy - mean(dy) - zh mean(dy zh))      written over ga (in place)
+// With s1 = s2 = 0 this is the eval-mode (frozen statistics) BatchNorm backward, dz = invstd gamma dy.
 __global__ void train_bn_bwd_apply_kernel(float *__restrict__ ga, const float *__restrict__ z, const float *__restrict__ mean,
                                           const float *__restrict__ invstd, const float *__restrict__ gamma,
                                           const float *__restrict__ beta, const float *__restrict__ s1,
@@ -351,6 +372,46 @@ __global__ void train_upsample_adjoint_kernel(const float *__restrict__ din, flo
         if (i1 == m) acc = fmaf(lam1, d, acc);
     }
     g_prev[i] = acc;
+}
+
+// gradient of the network input x [B][1][T]: the head's raw-input channel (model/unet_basic.py:98-99) plus the input gradient
+// of block 0 (Cin = 1, a transposed convolution of dz0 = the block's dz):
+//   dx[b][t] = Wo[C] dy (1 - y^2) + sum_co sum_k w0[co][0][k] dz0[b][co][t + PAD - k]
+// One thread per sample; each step of the channel loop stages IN_CH channels of a dz0 tile with its KS - 1 halo and their
+// weights in shared memory, so dz0 is read once. fp32 at both training precisions (block 0 always runs fp32).
+template <int KS>
+__global__ void __launch_bounds__(256) train_input_grad_kernel(const float *__restrict__ dz0, const float *__restrict__ w0,
+                                                               const float *__restrict__ dy, const float *__restrict__ y,
+                                                               const float *__restrict__ wo, float *__restrict__ dx, int C0,
+                                                               int C, int T)
+{
+    constexpr int PAD = (KS - 1) / 2, TILE = 256, IN_CH = 8, W = TILE + KS - 1;
+    __shared__ float ds[IN_CH][W];
+    __shared__ float ws[IN_CH][KS];
+    const int tid = threadIdx.x, b = blockIdx.y;
+    const int l0 = blockIdx.x * TILE, l = l0 + tid;
+    float acc = 0.f;
+    for (int c0 = 0; c0 < C0; c0 += IN_CH) {
+        __syncthreads();
+        for (int i = tid; i < IN_CH * W; i += TILE) {
+            const int c = i / W, j = i - c * W, p = l0 - PAD + j;
+            ds[c][j] = (c0 + c < C0 && p >= 0 && p < T) ? __ldg(dz0 + ((size_t)b * C0 + c0 + c) * T + p) : 0.f;
+        }
+        if (tid < IN_CH * KS) {
+            const int c = tid / KS, k = tid - c * KS;
+            ws[c][k] = c0 + c < C0 ? __ldg(w0 + (size_t)(c0 + c) * KS + k) : 0.f;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int c = 0; c < IN_CH; ++c)
+#pragma unroll
+            for (int k = 0; k < KS; ++k) acc = fmaf(ds[c][tid + 2 * PAD - k], ws[c][k], acc);
+    }
+    if (l < T) {
+        const size_t i = (size_t)b * T + l;
+        const float yv = y[i];
+        dx[i] = fmaf(wo[C], dy[i] * (1.f - yv * yv), acc);
+    }
 }
 
 // both packings of a block's weights, every step (the parameters change every step):
@@ -545,16 +606,18 @@ size_t train_workspace_bytes(int n, int ci, int B, int T, int prec)
 }
 
 int train_forward(int n, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum, void *workspace,
-                  cudaStream_t st, int prec)
+                  cudaStream_t st, int prec, int flags)
 {
+    const bool frozen = flags & TRAIN_FROZEN_BN;
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
     layout_of(sh, B, lo, prec);
     float *ws = static_cast<float *>(workspace);
     const bool naive = train_naive() && prec == TRAIN_FP32;
-    if (sh[0].cout * (2 * n) > kMaxC && !naive) return train_fail("channel plan too wide for the training kernels (%d channels)", sh[0].cout * 2 * n);
-    if (!naive) {
+    // the ones / zeros vectors serve the linear conv epilogue and, as s1 = s2 = 0, the frozen-statistics BatchNorm backward
+    if (sh[0].cout * (2 * n) > kMaxC && (!naive || frozen)) return train_fail("channel plan too wide for the training kernels (%d channels)", sh[0].cout * 2 * n);
+    if (!naive || frozen) {
         train_fill_kernel<<<(kMaxC + 255) / 256, 256, 0, st>>>(ws + lo.ones, 1.f, kMaxC);
         train_fill_kernel<<<(kMaxC + 255) / 256, 256, 0, st>>>(ws + lo.zeros, 0.f, kMaxC);
     }
@@ -578,8 +641,12 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
         } else if (s.mode == SRC_DIRECT) train_conv_fwd_kernel<15, SRC_DIRECT><<<grid, 128, 0, st>>>(a, P.conv_w[i], P.conv_b[i], z);
         else if (s.mode == SRC_DECIM) train_conv_fwd_kernel<15, SRC_DECIM><<<grid, 128, 0, st>>>(a, P.conv_w[i], P.conv_b[i], z);
         else train_conv_fwd_kernel<5, SRC_UPCAT><<<grid, 128, 0, st>>>(a, P.conv_w[i], P.conv_b[i], z);
-        train_bn_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, momentum, ws + lo.mean[i], ws + lo.invstd[i],
-                                                                 P.bn_mean[i], P.bn_var[i]);
+        if (frozen)
+            train_bn_frozen_stats_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(P.bn_mean[i], P.bn_var[i], ws + lo.mean[i],
+                                                                                   ws + lo.invstd[i], s.cout);
+        else
+            train_bn_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, momentum, ws + lo.mean[i], ws + lo.invstd[i],
+                                                                     P.bn_mean[i], P.bn_var[i]);
         const long long nel = (long long)B * s.cout * s.L;
         train_bn_act_kernel<<<blocks_for(nel, 256), 256, 0, st>>>(z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
                                                                   ws + lo.act[i], B, s.cout, s.L);
@@ -592,7 +659,7 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
 }
 
 int train_backward(int n, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
-                   const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec)
+                   const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec, float *dx, int flags)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
@@ -601,12 +668,16 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
     float *ws = static_cast<float *>(workspace);
     const int last = 2 * n, C = sh[last].cout;
     const bool naive = train_naive() && prec == TRAIN_FP32;
+    const bool frozen = flags & TRAIN_FROZEN_BN, pgrads = !(flags & TRAIN_NO_PARAM_GRADS);
     if (part < -1 || part > 1) return train_fail("training backward: part must be -1, 0 or 1 (got %d)", part);
+    if (dx && part == 0) return train_fail("training backward: dx is written by part 1 (or -1), not part 0");
     if (part != 1) {
-        cudaMemsetAsync(G.out_w, 0, (C + 1) * sizeof(float), st);
-        cudaMemsetAsync(G.out_b, 0, sizeof(float), st);
+        if (pgrads) {
+            cudaMemsetAsync(G.out_w, 0, (C + 1) * sizeof(float), st);
+            cudaMemsetAsync(G.out_b, 0, sizeof(float), st);
+        }
         train_head_bwd_kernel<<<blocks_for((long long)B * T, 256), 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last],
-                                                                                 G.out_w, G.out_b, B, C, T);
+                                                                                 pgrads ? G.out_w : nullptr, G.out_b, B, C, T);
     }
     const int i_hi = (part == 1) ? n : last, i_lo = (part == 0) ? n + 1 : 0;
     for (int i = i_hi; i >= i_lo; --i) {
@@ -614,22 +685,29 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         float *ga = ws + lo.ga[i];                               // gradient of the activation; becomes dz in place
         const float *z = ws + lo.z[i];
         const long long nel = (long long)B * s.cout * s.L;
-        train_bn_bwd_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
-                                                                     G.bn_w[i], G.bn_b[i], ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);
+        // batch statistics: dz needs mean(dy) and mean(dy zh) (s1, s2); frozen statistics: they are constants, dz = invstd
+        // gamma dy (s1 = s2 = 0), and the reductions only serve the BatchNorm parameter gradients
+        if (!frozen || pgrads)
+            train_bn_bwd_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
+                                                                         pgrads ? G.bn_w[i] : nullptr, pgrads ? G.bn_b[i] : nullptr,
+                                                                         ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);
+        const float *s1 = frozen ? ws + lo.zeros : ws + lo.s1[i], *s2 = frozen ? ws + lo.zeros : ws + lo.s2[i];
         train_bn_bwd_apply_kernel<<<blocks_for(nel, 256), 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
-                                                                        ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);
-        train_channel_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, G.conv_b[i], B, s.cout, s.L);
-        // weight gradient
+                                                                        s1, s2, B, s.cout, s.L);
         const ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
-        cudaMemsetAsync(G.conv_w[i], 0, (size_t)s.cout * s.cin * s.k * sizeof(float), st);
-        const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
-        if (on_tc(prec, i)) {
-            if (launch_wgrad_bf16(a, ga, G.conv_w[i], s.k, s.mode, st) < 0) return train_fail("training backward, block %d: bf16 weight-gradient launch failed", i);
-        } else if (!naive) {
-            launch_wgrad_fp32(a, ga, G.conv_w[i], s.mode, st);
-        } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
-        else if (s.mode == SRC_DECIM) train_conv_bwd_weight_kernel<15, SRC_DECIM><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
-        else train_conv_bwd_weight_kernel<5, SRC_UPCAT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
+        if (pgrads) {
+            train_channel_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, G.conv_b[i], B, s.cout, s.L);
+            // weight gradient
+            cudaMemsetAsync(G.conv_w[i], 0, (size_t)s.cout * s.cin * s.k * sizeof(float), st);
+            const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
+            if (on_tc(prec, i)) {
+                if (launch_wgrad_bf16(a, ga, G.conv_w[i], s.k, s.mode, st) < 0) return train_fail("training backward, block %d: bf16 weight-gradient launch failed", i);
+            } else if (!naive) {
+                launch_wgrad_fp32(a, ga, G.conv_w[i], s.mode, st);
+            } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
+            else if (s.mode == SRC_DECIM) train_conv_bwd_weight_kernel<15, SRC_DECIM><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
+            else train_conv_bwd_weight_kernel<5, SRC_UPCAT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
+        }
         // input gradient and its routing to the producers of the block input
         if (s.mode != SRC_DIRECT) {
             float *din = ws + lo.din;
@@ -657,6 +735,13 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         }
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return train_fail("training backward, block %d: %s", i, cudaGetErrorString(e));
+    }
+    if (dx) {
+        // part -1 or 1: ga[0] now holds block 0's dz
+        const dim3 gx(blocks_for(T, 256), (unsigned)B);
+        train_input_grad_kernel<15><<<gx, 256, 0, st>>>(ws + lo.ga[0], P.conv_w[0], dy, y, P.out_w, dx, sh[0].cout, C, T);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return train_fail("training backward, input gradient: %s", cudaGetErrorString(e));
     }
     return 0;
 }

@@ -26,17 +26,24 @@ struct TrainGrads {
 // dz; round to nearest), fp32 accumulation on the tensor cores (wunet_train_tc.cu); the first block stays fp32. Everything else
 // is fp32 at both precisions. The workspace of TRAIN_BF16 is the fp32 one plus the bf16 weight packings.
 enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1 };
+// TRAIN_FROZEN_BN: BatchNorm normalises by the running statistics and never updates them (eval-mode BatchNorm); the forward
+// and the backward of one step must agree on it. TRAIN_NO_PARAM_GRADS (backward only): no parameter gradient is computed
+// (G may hold null pointers), only the input gradient.
+enum TrainFlags : int { TRAIN_FROZEN_BN = 1, TRAIN_NO_PARAM_GRADS = 2 };
 
 const char *train_error();
 size_t train_workspace_bytes(int n_layers, int ci, int B, int T, int prec = TRAIN_FP32);
-// y = model(x) with BatchNorm in training mode; keeps every pre-BN output and activation in `workspace` for the backward
+// y = model(x) with BatchNorm in training mode (or, with TRAIN_FROZEN_BN, eval mode); keeps every pre-BN output and
+// activation in `workspace` for the backward
 int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum,
-                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32);
+                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32, int flags = 0);
 // gradients of every parameter for the upstream gradient dy of the output; `workspace` as left by train_forward.
 // part: -1 = the whole backward; 0 = head + decoder blocks (their gradients are complete afterwards: a data-parallel caller
 // starts reducing them while part 1 runs); 1 = middle + encoder blocks (must follow part 0 on the same stream).
+// dx (optional, [B][1][T], fully overwritten): gradient of the input x; written by part -1 or 1 (block 0 is in part 1).
 int train_backward(int n_layers, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
-                   const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1, int prec = TRAIN_FP32);
+                   const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1, int prec = TRAIN_FP32,
+                   float *dx = nullptr, int flags = 0);
 // One convolution-shaped pass on caller device buffers (test hook): pass 0 = forward conv out[B][Cout][L] = conv(in, w);
 // 1 = input gradient out[B][Cin][L] of dz [B][Cout][L] (Conv1d padding, no mode); 2 = weight gradient out[Cout][Cin][K] =
 // sum dz * in. `in` is built from src0 / src1 per `mode` as in the forward (ConvArgs). Synchronous.

@@ -131,16 +131,21 @@ class _NativeState:
 
 
 class _NativeTrainStep(torch.autograd.Function):
-    """forward = wunet_train_forward, backward = wunet_train_backward (include/wunet_b200.h). The activations live in a
+    """forward = wunet_train_forward_ex, backward = wunet_train_backward_ex (include/wunet_b200.h). The activations live in a
     workspace tensor kept on the autograd context; parameter order: 4 per conv block (conv.weight, conv.bias, bn.weight,
-    bn.bias) in forward order, then out.weight, out.bias."""
+    bn.bias) in forward order, then out.weight, out.bias.
+
+    ``flags``: 0 = BatchNorm with batch statistics, running buffers updated (.train()); ``_lib.TRAIN_FROZEN_BN`` = BatchNorm
+    normalising by the running statistics, which stay untouched (.eval()). The backward fills the gradient of ``x`` when it
+    requires grad and those of the parameters when any of them does; with no parameter requiring grad it computes ``dx``
+    only (no weight-gradient pass, no reduction, no all-reduce)."""
 
     @staticmethod
     def _ptr_array(tensors):
         return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
 
     @staticmethod
-    def forward(ctx, model, x, *params):
+    def forward(ctx, model, flags, x, *params):
         lib = _lib.load()
         blocks = model._blocks()
         nb = len(blocks)
@@ -162,11 +167,12 @@ class _NativeTrainStep(torch.autograd.Function):
             momentum = float(blocks[0][1].momentum)
             stream = torch.cuda.current_stream(x.device).cuda_stream
             P = _NativeTrainStep._ptr_array
-            _lib.check(lib.wunet_train_forward_prec(c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b),
-                                                    P(rmean), P(rvar), params[-2].data_ptr(), params[-1].data_ptr(), momentum,
-                                                    ws.data_ptr(), ws.numel(), stream, prec))
-        # the backward runs at the precision of ITS forward (and reads the bf16 weight packings that forward left in ws)
-        ctx.model, ctx.ws, ctx.nb, ctx.prec = model, ws, nb, prec
+            _lib.check(lib.wunet_train_forward_ex(c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b),
+                                                  P(rmean), P(rvar), params[-2].data_ptr(), params[-1].data_ptr(), momentum,
+                                                  ws.data_ptr(), ws.numel(), stream, prec, flags))
+        # the backward runs at the precision and BatchNorm mode of ITS forward (and reads the bf16 weight packings that
+        # forward left in ws)
+        ctx.model, ctx.ws, ctx.nb, ctx.prec, ctx.flags = model, ws, nb, prec, flags
         ctx.save_for_backward(x, y, *params)
         return y
 
@@ -178,29 +184,38 @@ class _NativeTrainStep(torch.autograd.Function):
         nb = ctx.nb
         B, _, T = x.shape
         gy = gy.contiguous()
-        # all gradients live in ONE flat buffer laid out in backward-completion order (train_step.GradientBucket); autograd
-        # hands the views to .grad, so the all-reduce below needs no gather / scatter copies
-        bucket = GradientBucket([p.shape for p in params], nb, x.device)
-        grads = bucket.views
-        reduce = ctx.model.data_parallel != "off" and data_parallel_world() > 1
+        want_dx = ctx.needs_input_grad[2]
+        want_params = any(ctx.needs_input_grad[3:])
+        dx = torch.empty_like(x) if want_dx else None
+        flags = ctx.flags | (0 if want_params else _lib.TRAIN_NO_PARAM_GRADS)
+        if want_params:
+            # all gradients live in ONE flat buffer laid out in backward-completion order (train_step.GradientBucket); autograd
+            # hands the views to .grad, so the all-reduce below needs no gather / scatter copies
+            bucket = GradientBucket([p.shape for p in params], nb, x.device)
+            grads = bucket.views
+            reduce = ctx.model.data_parallel != "off" and data_parallel_world() > 1
+        else:
+            grads, reduce = [None] * len(params), False      # input gradient only: nothing to reduce (dx is per sample)
         with torch.cuda.device(x.device):
             c = ctx.model._context(x.device)
             stream = torch.cuda.current_stream(x.device).cuda_stream
             P = _NativeTrainStep._ptr_array
             sel = lambda ts, k: [ts[4 * i + k] for i in range(nb)]          # noqa: E731
+            G = (lambda k: P(sel(grads, k))) if want_params else (lambda k: None)   # noqa: E731
+            ptr = lambda t: None if t is None else t.data_ptr()               # noqa: E731
             for part in ((0, 1) if reduce else (-1,)):
-                _lib.check(lib.wunet_train_backward_part_prec(c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)),
-                                                              P(sel(params, 2)), P(sel(params, 3)), params[-2].data_ptr(),
-                                                              P(sel(grads, 0)), P(sel(grads, 1)), P(sel(grads, 2)), P(sel(grads, 3)),
-                                                              grads[-2].data_ptr(), grads[-1].data_ptr(), ctx.ws.data_ptr(),
-                                                              ctx.ws.numel(), stream, part, ctx.prec))
+                _lib.check(lib.wunet_train_backward_ex(c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)),
+                                                       P(sel(params, 2)), P(sel(params, 3)), params[-2].data_ptr(),
+                                                       G(0), G(1), G(2), G(3), ptr(grads[-2]), ptr(grads[-1]), ctx.ws.data_ptr(),
+                                                       ctx.ws.numel(), stream, ptr(dx) if part != 0 else None, part, ctx.prec,
+                                                       flags))
                 if reduce:
                     # head + decoder gradients are final after part 0: their all-reduce overlaps part 1 (middle + encoders)
                     bucket.reduce_part(part)
             if reduce:
                 bucket.finish()
         ctx.ws = None
-        return (None, None, *grads)                          # no gradient for the model handle and for the input
+        return (None, None, dx, *grads)                      # no gradient for the model handle and the flags
 
 
 class Model(nn.Module):
@@ -228,10 +243,22 @@ class Model(nn.Module):
                    BatchNorm, the head and all gradients stay fp32, parameters stay fp32 (the caller's optimizer is unchanged).
                    ``torch.autocast(bfloat16)`` semantics for Conv1d, except that z is kept in fp32. Only with
                    train_backend="native". Not part of the state_dict.
+    eval_autograd  when an eval-mode forward records an autograd graph (grad mode on, train_backend "native" or "torch").
+                   "input" (default): when the input requires grad — ``x.grad`` of an upstream model or front end, input
+                   gradients of an adversarial perturbation. "always": also when some parameter requires grad, for
+                   fine-tuning with frozen BatchNorm statistics (``model.eval()`` then ``loss.backward()``). "off": the eval
+                   forward always returns a detached tensor. A recorded eval forward runs the native training kernels at
+                   ``train_precision`` with BatchNorm normalising by the running statistics, which it leaves untouched (the
+                   reference's eval-mode BatchNorm), and keeps the activations for the backward; gradients reach ``x`` and
+                   every parameter that requires grad, averaged over data-parallel ranks like the training backward. Every
+                   other eval forward takes the inference kernels (``precision``) and returns a detached tensor. "always" is
+                   not the default because a caller that runs inference without ``torch.no_grad()`` (enhancement.py:66) would
+                   then pay for the training kernels and their workspace on every call. Not part of the state_dict.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
-                 train_backend: str = "native", data_parallel: str = "auto", train_precision: str = "fp32"):
+                 train_backend: str = "native", data_parallel: str = "auto", train_precision: str = "fp32",
+                 eval_autograd: str = "input"):
         super().__init__()
         if precision not in _lib.PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(_lib.PRECISIONS)}, got {precision!r}")
@@ -245,10 +272,13 @@ class Model(nn.Module):
             raise ValueError(f"train_precision must be 'fp32' or 'bf16', got {train_precision!r}")
         if train_precision != "fp32" and train_backend != "native":
             raise ValueError(f"train_precision={train_precision!r} needs train_backend='native' (got {train_backend!r})")
+        if eval_autograd not in ("input", "always", "off"):
+            raise ValueError(f"eval_autograd must be 'input', 'always' or 'off', got {eval_autograd!r}")
         self.precision = precision
         self.train_backend = train_backend
         self.data_parallel = data_parallel
         self.train_precision = train_precision
+        self.eval_autograd = eval_autograd
         n, ci = n_layers, channels_interval
 
         enc_in = [1] + [i * ci for i in range(1, n)]
@@ -335,21 +365,36 @@ class Model(nn.Module):
             raise NotImplementedError(
                 "this model was built with train_backend='none': call model.eval(), or construct it with "
                 "train_backend='native' (default; sm_90a kernels) or 'torch' (composite PyTorch path).")
-        # eval mode: like enhancement.py:66 (`model(chunk).detach().cpu()`, no torch.no_grad()) the result is
-        # returned detached — the native path records no autograd graph.
+        # eval mode: a forward that needs a graph (see eval_autograd: the input requires grad, or "always" and a parameter
+        # does) runs the training kernels with eval-mode BatchNorm, or the composite path for train_backend="torch".
+        # Everything else — enhancement.py:66 (`model(chunk).detach().cpu()`, no torch.no_grad()), validation under
+        # torch.no_grad(), an empty batch — takes the inference kernels and gets a detached result.
+        if input.numel() != 0 and self._eval_records_graph(input):
+            if self.train_backend == "native":
+                return self._forward_train_native(input, frozen_bn=True)
+            return self._forward_torch_reference_semantics(input)
         return self._forward_native(input)
+
+    def _eval_records_graph(self, x: torch.Tensor) -> bool:
+        if self.eval_autograd == "off" or self.train_backend == "none" or not torch.is_grad_enabled():
+            return False
+        if x.requires_grad:
+            return True
+        return self.eval_autograd == "always" and any(p.requires_grad for p in self.parameters())
 
     @property
     def reduces_gradients(self) -> bool:
         """True when ``loss.backward()`` through this model already averages the gradients over the data-parallel ranks."""
         from .train_step import data_parallel_world
-        return (self.training and self.train_backend == "native" and self.data_parallel != "off"
-                and data_parallel_world() > 1)
+        return ((self.training or self.eval_autograd != "off") and self.train_backend == "native"
+                and self.data_parallel != "off" and data_parallel_world() > 1)
 
-    def _forward_train_native(self, x: torch.Tensor) -> torch.Tensor:
-        """Training-mode forward through libwunet_b200 (wunet_train_forward / wunet_train_backward behind a
-        torch.autograd.Function): BatchNorm uses batch statistics and updates its running buffers, ``loss.backward()`` fills
-        ``.grad`` of all 102 parameters, the caller's optimizer is used unchanged (trainer/trainer.py:34-38). fp32 or, with
+    def _forward_train_native(self, x: torch.Tensor, frozen_bn: bool = False) -> torch.Tensor:
+        """Training-kernel forward through libwunet_b200 (wunet_train_forward_ex / wunet_train_backward_ex behind a
+        torch.autograd.Function): ``loss.backward()`` fills ``.grad`` of the parameters that require grad (all 102 in
+        training) and of ``x`` when it requires grad; the caller's optimizer is used unchanged (trainer/trainer.py:34-38).
+        BatchNorm uses batch statistics and updates its running buffers (.train()) or, with ``frozen_bn``, normalises by the
+        running statistics and leaves them and ``num_batches_tracked`` untouched (.eval()). fp32 or, with
         ``train_precision="bf16"``, bf16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
         if not x.is_cuda:
@@ -363,7 +408,9 @@ class Model(nn.Module):
         for t in params:
             if t.device != x.device or t.dtype != torch.float32 or not t.is_contiguous():
                 raise RuntimeError("libwunet_b200 needs contiguous float32 parameters on the input's device")
-        y = _NativeTrainStep.apply(self, self._aligned(x), *params)
+        y = _NativeTrainStep.apply(self, _lib.TRAIN_FROZEN_BN if frozen_bn else 0, self._aligned(x), *params)
+        if frozen_bn:
+            return y                                         # running statistics untouched: the folded copies stay valid
         for blk in blocks:                                   # torch.nn.BatchNorm1d bookkeeping (momentum is not None: unused)
             blk[1].num_batches_tracked += 1
         # the kernels updated running_mean / running_var through raw pointers (no _version bump): drop the folded copies
