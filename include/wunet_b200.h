@@ -220,6 +220,8 @@ int wunet_train_backward_part_prec(wunet_ctx *ctx, const float *x, const float *
 /* wunet_train_forward_ex: with WUNET_TRAIN_FROZEN_BN, BatchNorm normalises by bn_running_mean / bn_running_var, which are only
  *   read (momentum is unused): model/unet_basic.py in .eval() mode, with the activations kept for the backward. The forward
  *   ignores WUNET_TRAIN_NO_PARAM_GRADS. The workspace size is wunet_train_workspace_bytes_prec (frozen mode needs nothing extra).
+ *   Batch statistics of one value per channel (B = 1 and T = 2^n_layers: L = 1 at the middle block) -> WUNET_EINVAL, where
+ *   torch.nn.BatchNorm1d raises in training mode; with WUNET_TRAIN_FROZEN_BN that shape is accepted.
  * wunet_train_backward_ex: dx [B][1][T] (device, or NULL) is fully overwritten with the gradient of x. It belongs to part 1
  *   (block 0 is there): pass it with part -1 or 1; dx with part 0 is WUNET_EINVAL. With WUNET_TRAIN_NO_PARAM_GRADS no weight
  *   gradient, bias or BatchNorm-parameter reduction runs and nothing is written through g_*.
@@ -246,6 +248,22 @@ int wunet_train_backward_ex(wunet_ctx *ctx, const float *x, const float *y, cons
  * No reference counterpart (autograd computes these inside loss.backward(), trainer/trainer.py:37). */
 int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, int L, int cin0, int cin1, int cout,
                            const float *src0, const float *src1, const float *w, const float *dz, float *out);
+
+/* Introspection for tests, host-only (needs no GPU, no context): the training step of an n_layers / channels_interval model at
+ * batch B, frame length T and training `precision` (WUNET_PREC_FP32 or WUNET_PREC_BF16), block `block` (0 .. 2*n_layers, forward
+ * order). Writes 22 long longs (capacity >= 22):
+ *  [0] z  [1] act  [2] ga  [3] mean  [4] invstd  [5] s1  [6] s2: byte offsets in the training workspace of the block's pre-BatchNorm
+ *      output z [B][Cout][L], its activation [B][Cout][L], the activation gradient [B][Cout][L] (which holds dz after the
+ *      backward), and the fp32 [Cout] vectors of the BatchNorm mean and 1/sqrt(var + eps) used by the forward and of the
+ *      backward's mean(dy) and mean(dy * zhat) (written when that reduction runs)
+ *  [7] Cin  [8] Cin0  [9] Cin1 (the skip channels of a decoder)  [10] Cout  [11] L  [12] ksize  [13] input mode (0 = the raw input,
+ *      1 = the previous activation decimated, 2 = interpolated previous activation + skip)
+ *  [14] weight-gradient kernel (0 = fp32 tiled, 1 = bf16 wgmma; block 0 is always 0)  [15] [16] [17] its gridDim x, y, z
+ *  [18] (frame, position tile) work items shared by the gridDim.z slices  [19] positions per item  [20] largest number of items
+ *      one CTA reduces  [21] wunet_train_workspace_bytes_prec for this B, T and precision.
+ * No reference counterpart. */
+int wunet_debug_train_layout(int n_layers, int channels_interval, int B, int T, int precision, int block, long long *fields,
+                             int capacity);
 
 /* Introspection for tests and tuning, host-only (needs no GPU, no context): the tiling the bf16 path would use for conv
  * block `block` (1 .. 2*n_layers; block 0 = first encoder runs on CUDA cores) at batch B, frame length T, on a device with

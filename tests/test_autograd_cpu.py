@@ -121,3 +121,21 @@ def test_input_requiring_grad_records_a_graph_on_the_torch_backend(monkeypatch):
     m(x).sum().backward()
     assert not calls
     assert x.grad is not None and x.grad.shape == x.shape
+
+
+@pytest.mark.parametrize("n,ci", [(12, 24), (4, 8)])
+def test_one_value_per_channel_raises_like_batchnorm(n, ci):
+    """Training mode, B = 1, T = 2^n_layers: the middle block sees one value per channel and torch.nn.BatchNorm1d raises its
+    ValueError. The native backend raises the same error before it needs a GPU; eval mode (running statistics) accepts it."""
+    x = torch.zeros(1, 1, 1 << n)
+    msgs = []
+    for backend in ("torch", "native"):
+        m = Model(n, ci, train_backend=backend).train()
+        with pytest.raises(ValueError, match="Expected more than 1 value per channel when training") as e:
+            m(x)
+        msgs.append(str(e.value))
+    assert msgs[0] == msgs[1]
+    m = Model(n, ci, train_backend="torch").eval()
+    assert m(x.clone().requires_grad_(True)).shape == x.shape
+    with pytest.raises(RuntimeError, match="no CPU fallback"):
+        Model(n, ci).train()(torch.zeros(1, 1, 2 << n))           # two values per channel: on to the device check

@@ -5,7 +5,8 @@ composite PyTorch path.
 
 Bars: training mode keeps the bars of test_train_gpu.py (fp32) and test_train_bf16_gpu.py (bf16: max(2 x autocast's error,
 the fp32 bar)); the input gradient is held to the same bar as the parameter gradients. Eval mode has no batch statistics to
-amplify rounding, so its output is held to 1e-4 max-abs and its loss to 1e-5 relative.
+amplify rounding, so its output is held to 1e-4 max-abs, its loss to 1e-5 relative and, at the full architecture, its
+gradients to 2e-5 of their largest entry.
 
 Not covered here: data parallel (two GPUs). The eval-mode backward averages the parameter gradients through the same
 GradientBucket path as the training backward, which test_ddp_gpu.py covers."""
@@ -22,8 +23,10 @@ pytestmark = [pytest.mark.gpu]
 
 SMALL, FULL = "autograd_small_n4_c8.npz", "autograd_full_n12_c24_b2_t4096.npz"
 # (loss relative, output max-abs, worst gradient relative to its largest entry) of the fp32 native step
+# Eval mode has no batch statistics to amplify rounding: the full architecture's worst gradient is 1.3e-6 and dx 1.7e-6 from
+# float64 (H100 80GB HBM3, 700 W), so its bar sits about 10x above that instead of at the training step's 2e-2.
 FP32_BARS = {(SMALL, "train"): (1e-5, 1e-5, 2e-4), (FULL, "train"): (1e-4, 1e-3, 2e-2),
-             (SMALL, "eval"): (1e-5, 1e-4, 2e-4), (FULL, "eval"): (1e-5, 1e-4, 2e-2)}
+             (SMALL, "eval"): (1e-5, 1e-4, 2e-4), (FULL, "eval"): (1e-5, 1e-4, 2e-5)}
 
 
 def make_pair(B, T, seed):
@@ -261,7 +264,8 @@ def test_cascade_trains_the_upstream_model(monkeypatch):
 
 def test_frozen_batchnorm_fine_tuning_step(monkeypatch):
     """eval_autograd="always", model.eval(), plain input: one fine-tuning step with frozen BatchNorm statistics, reference
-    architecture at T = 16384, B = 4, native against the composite path (no TF32); running statistics untouched."""
+    architecture at T = 16384, B = 4, native against the composite path (no TF32); running statistics untouched. Nothing
+    amplifies rounding here: the worst gradient differs by 5.4e-6 of its largest entry (H100 80GB HBM3, 700 W), held to 6e-5."""
     monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     n, ci, B, T = 12, 24, 4, 16384
@@ -280,4 +284,4 @@ def test_frozen_batchnorm_fine_tuning_step(monkeypatch):
     loss_e = abs(models["native"][1] - models["torch"][1]) / models["torch"][1]
     print(f"frozen-BN fine-tuning: loss rel diff {loss_e:.2e}, worst gradient rel diff native vs composite {worst[0]:.2e} ({worst[1]})")
     assert loss_e <= 1e-5
-    assert worst[0] <= 2e-2, worst
+    assert worst[0] <= 6e-5, worst

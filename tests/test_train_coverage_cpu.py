@@ -1,0 +1,113 @@
+"""The teacher-forced training check (tests/test_train_blocks_gpu.py) only means something if its cases reach the regimes where
+the training kernels can go wrong. This guard reads its case table through the host-only layout query (no GPU needed):
+every block's workspace regions are sound, and together the cases reach
+
+- the fp32 weight gradient with >= 32 tiles per CTA (the tile loop) and with exactly one;
+- the bf16 weight gradient with >= 100 items per CTA and with exactly one;
+- a frame whose last 128-position (fp32) or 64-position (bf16) tile is partial;
+- frames of fewer than 4 samples (the zero padding of the fp32 weight gradient's 4-position inner step);
+- Cout not a multiple of 16 and Cin not a multiple of 64 (partial co / ci tiles);
+- B = 1, frozen BatchNorm, a backward without parameter gradients, and the part 0 / part 1 split.
+
+It fails as soon as a change of the case table or of the launch geometry drops one of them."""
+import ctypes
+
+import pytest
+
+import test_train_blocks_gpu as blocks
+from wave_u_net_for_speech_enhancement_b200 import _lib
+
+REQUIRED = {"fp32_wgrad_ge_32_per_cta", "fp32_wgrad_1_per_cta", "bf16_wgrad_ge_100_per_cta", "bf16_wgrad_1_per_cta",
+            "partial_tile", "frame_lt_4", "cout_not_mult_16", "cin_not_mult_64", "batch_1", "frozen", "no_param_grads",
+            "part_split"}
+FIELDS = ("z", "act", "ga", "mean", "invstd", "s1", "s2")
+
+
+def regions(d, B):
+    big = 4 * B * d["Cout"] * d["L"]
+    return [(d[f], big if f in ("z", "act", "ga") else 4 * d["Cout"]) for f in FIELDS]
+
+
+def layouts(case, prec):
+    c = blocks.CASES[case]
+    return [_lib.debug_train_layout(c["n"], c["ci"], c["B"], c["T"], i, prec) for i in range(2 * c["n"] + 1)]
+
+
+@pytest.mark.parametrize("case", sorted(blocks.CASES))
+def test_layout_regions_are_disjoint_aligned_and_inside_the_workspace(case):
+    c = blocks.CASES[case]
+    for prec in ("fp32", "bf16"):
+        lay = layouts(case, prec)
+        total = lay[0]["workspace_bytes"]
+        spans = []
+        for i, d in enumerate(lay):
+            assert d["workspace_bytes"] == total
+            for off, size in regions(d, c["B"]):
+                assert off % 256 == 0 and 0 <= off and off + size <= total, (case, prec, i, off, size, total)
+                spans.append((off, off + size))
+        spans.sort()
+        assert all(a[1] <= b[0] for a, b in zip(spans, spans[1:])), (case, prec)
+    fp32, bf16 = layouts(case, "fp32"), layouts(case, "bf16")
+    for a, b in zip(fp32, bf16):
+        assert {f: a[f] for f in FIELDS} == {f: b[f] for f in FIELDS}
+    assert fp32[0]["workspace_bytes"] <= bf16[0]["workspace_bytes"]
+
+
+def test_layout_query_describes_the_channel_plan_and_the_weight_gradient_launch():
+    n, ci, B, T = 12, 24, 120, 16384
+    for prec in ("fp32", "bf16"):
+        for i in range(2 * n + 1):
+            d = _lib.debug_train_layout(n, ci, B, T, i, prec)
+            L = T >> i if i <= n else T >> (2 * n - i)
+            assert (d["L"], d["ksize"], d["mode"]) == (L, 15 if i <= n else 5, 0 if i == 0 else 1 if i <= n else 2)
+            assert d["Cin"] == d["Cin0"] + d["Cin1"] and (d["Cin1"] > 0) == (i > n)
+            assert d["wgrad_tc"] == (1 if prec == "bf16" and i > 0 else 0)
+            tiles = -(-L // d["positions"])
+            assert d["items"] == B * tiles and d["items_per_cta"] == -(-d["items"] // d["grid_z"])
+            if d["wgrad_tc"]:
+                assert d["positions"] == 64 and d["grid_x"] == -(-d["Cout"] // 64) * (d["ksize"] // 5)
+            else:
+                assert d["positions"] == min(L, 128) and (d["grid_x"], d["grid_y"]) == (-(-d["Cout"] // 16), -(-d["Cin"] // 64))
+    fp32 = [_lib.debug_train_layout(n, ci, B, T, i, "fp32")["items_per_cta"] for i in range(2 * n + 1)]
+    bf16 = [_lib.debug_train_layout(n, ci, B, T, i, "bf16")["items_per_cta"] for i in range(1, 2 * n + 1)]
+    assert (min(fp32), max(fp32), min(bf16), max(bf16)) == (4, 52, 14, 233)
+    for bad in [(12, 24, 2, 4096, 25, "fp32"), (12, 24, 2, 4000, 0, "fp32"), (12, 24, 2, 4096, 0, "fp32_tc")]:
+        with pytest.raises(_lib.WunetError):
+            _lib.debug_train_layout(*bad)
+    buf = (ctypes.c_longlong * 4)()
+    assert _lib.load().wunet_debug_train_layout(12, 24, 2, 4096, _lib.PREC_FP32, 0, buf, 4) != 0
+
+
+def features(case, prec, mode, pgrads):
+    c = blocks.CASES[case]
+    f = set()
+    for d in layouts(case, prec):
+        kind = "bf16" if d["wgrad_tc"] else "fp32"
+        if d["items_per_cta"] == 1:
+            f.add(f"{kind}_wgrad_1_per_cta")
+        if d["items_per_cta"] >= (100 if kind == "bf16" else 32):
+            f.add(f"{kind}_wgrad_ge_{100 if kind == 'bf16' else 32}_per_cta")
+        if d["L"] % d["positions"] != 0:
+            f.add("partial_tile")
+        if d["L"] < 4:
+            f.add("frame_lt_4")
+        if d["Cout"] % 16 != 0:
+            f.add("cout_not_mult_16")
+        if d["Cin"] % 64 != 0:
+            f.add("cin_not_mult_64")
+    if c["B"] == 1:
+        f.add("batch_1")
+    if mode == "frozen":
+        f.add("frozen")
+    if not pgrads:
+        f.add("no_param_grads")
+    if (case, prec) in blocks.SPLIT:
+        f.add("part_split")
+    return f
+
+
+def test_cases_reach_every_training_regime():
+    got = set()
+    for case, prec, mode, pgrads in blocks.RUNS:
+        got |= features(case, prec, mode, pgrads)
+    assert REQUIRED <= got, f"no case reaches {sorted(REQUIRED - got)}"

@@ -73,6 +73,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_forward_ex.argtypes = lib.wunet_train_forward_prec.argtypes + [ci]
     lib.wunet_train_backward_ex.argtypes = lib.wunet_train_backward.argtypes + [vp, ci, ci, ci]
     lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
+    lib.wunet_debug_train_layout.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ll), ci]
     _lib = lib
     return lib
 
@@ -89,7 +90,7 @@ EXPORTED_SYMBOLS = [
     "wunet_debug_pair_weights",
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
-    "wunet_train_forward_ex", "wunet_train_backward_ex",
+    "wunet_train_forward_ex", "wunet_train_backward_ex", "wunet_debug_train_layout",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]
@@ -105,3 +106,16 @@ def debug_plan(n_layers: int, channels_interval: int, B: int, T: int, block: int
     buf = (ctypes.c_int * 32)()
     check(load().wunet_debug_plan_prec(n_layers, channels_interval, B, T, block, num_sms, buf, 32, PRECISIONS[precision]))
     return dict(zip(PLAN_FIELDS, [int(v) for v in buf]))
+
+
+TRAIN_LAYOUT_FIELDS = ["z", "act", "ga", "mean", "invstd", "s1", "s2", "Cin", "Cin0", "Cin1", "Cout", "L", "ksize", "mode",
+                       "wgrad_tc", "grid_x", "grid_y", "grid_z", "items", "positions", "items_per_cta", "workspace_bytes"]
+
+
+def debug_train_layout(n_layers: int, channels_interval: int, B: int, T: int, block: int, precision: str = "fp32") -> dict:
+    """Where one block's tensors live in the training workspace (byte offsets) and how its weight gradient is launched
+    (host-only query: works without a GPU)."""
+    n = len(TRAIN_LAYOUT_FIELDS)
+    buf = (ctypes.c_longlong * n)()
+    check(load().wunet_debug_train_layout(n_layers, channels_interval, B, T, PRECISIONS[precision], block, buf, n))
+    return dict(zip(TRAIN_LAYOUT_FIELDS, [int(v) for v in buf]))

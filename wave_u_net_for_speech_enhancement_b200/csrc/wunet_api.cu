@@ -509,6 +509,11 @@ int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T,
     const int prec = train_prec(precision);
     if (prec < 0) return WUNET_EINVAL;
     if (flags & ~kTrainFlags) return fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
+    // batch statistics of one value per channel (B = 1 and L = 1 at the middle block): torch.nn.BatchNorm1d raises in training
+    // mode rather than normalise by a variance of 0
+    if (!(flags & WUNET_TRAIN_FROZEN_BN) && B == 1 && (T >> c->n) == 1)
+        return fail(WUNET_EINVAL, "Expected more than 1 value per channel when training (B=1, T=%d: one value per channel at the "
+                                  "middle block)", T);
     if (!x || !y || !workspace || !conv_w || !conv_b || !bn_weight || !bn_bias || !bn_running_mean || !bn_running_var || !out_w || !out_b)
         return fail(WUNET_EINVAL, "null argument");
     const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
@@ -583,6 +588,18 @@ int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, 
     const int prec = train_prec(precision);
     if (prec < 0) return WUNET_EINVAL;
     if (train_debug_conv(pass, prec, mode, ksize, B, L, cin0, cin1, cout, src0, src1, w, dz, out))
+        return fail(WUNET_EINVAL, "%s", train_error());
+    return WUNET_OK;
+}
+
+int wunet_debug_train_layout(int n_layers, int channels_interval, int B, int T, int precision, int block, long long *fields,
+                             int capacity)
+{
+    if (n_layers < 1 || n_layers > 16 || channels_interval < 1 || B < 1 || T < 1 || (T % (1 << n_layers)) != 0)
+        return fail(WUNET_EINVAL, "bad training layout query");
+    const int prec = train_prec(precision);
+    if (prec < 0) return WUNET_EINVAL;
+    if (train_debug_layout(n_layers, channels_interval, B, T, prec, block, fields, capacity))
         return fail(WUNET_EINVAL, "%s", train_error());
     return WUNET_OK;
 }

@@ -80,6 +80,11 @@ int launch_pack_fp32(const float *w, const float *bias, const float *g, const fl
 int launch_conv_bf16(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
 // dw[co][ci][k] += sum_{b,l} dz[b][co][l] * in(b, ci, l + k - pad), in read through `a` as the forward reads it (dw zeroed first)
 int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st);
+// Launch geometry of the two weight-gradient kernels, the one definition their launchers and wunet_debug_train_layout use:
+// grid, number of (frame, position tile) work items that gridDim.z slices share, and positions per item.
+struct WgradGrid { dim3 grid; int items, positions; };
+WgradGrid wgrad_grid_fp32(int B, int L, int Cin, int Cout);             // train_wgrad_kernel (wunet_train.cu)
+WgradGrid wgrad_grid_bf16(int B, int L, int Cin, int Cout, int ksize);  // train_wgrad_tc_kernel (wunet_train_tc.cu)
 // bf16 elements of one packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout))
 size_t train_tc_packed_elems(int cout, int cin, int k);
 int train_tc_pack(const float *w, __nv_bfloat16 *wf, __nv_bfloat16 *wb, int Cout, int Cin, int K, cudaStream_t st);

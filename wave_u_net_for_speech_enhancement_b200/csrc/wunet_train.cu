@@ -507,14 +507,10 @@ __global__ void __launch_bounds__(256) train_wgrad_kernel(const ConvArgs a, cons
 // the tiled fp32 weight gradient (dw zeroed first); mode DIRECT / DECIM: 15 taps, UPCAT: 5
 void launch_wgrad_fp32(const ConvArgs &a, const float *dz, float *dw, int mode, cudaStream_t st)
 {
-    const int lt = std::min(a.L, 128);
-    const int nco = (a.Cout + 15) / 16, nci = (a.Cin + 63) / 64;
-    const int ntiles = a.B * ((a.L + lt - 1) / lt);
-    const int slices = std::max(1, std::min(ntiles, 1184 / (nco * nci)));           // ~4 blocks per SM over the grid
-    const dim3 gt((unsigned)nco, (unsigned)nci, (unsigned)slices);
-    if (mode == SRC_DIRECT) train_wgrad_kernel<15, SRC_DIRECT><<<gt, 256, 0, st>>>(a, dz, dw, lt);
-    else if (mode == SRC_DECIM) train_wgrad_kernel<15, SRC_DECIM><<<gt, 256, 0, st>>>(a, dz, dw, lt);
-    else train_wgrad_kernel<5, SRC_UPCAT><<<gt, 256, 0, st>>>(a, dz, dw, lt);
+    const WgradGrid g = wgrad_grid_fp32(a.B, a.L, a.Cin, a.Cout);
+    if (mode == SRC_DIRECT) train_wgrad_kernel<15, SRC_DIRECT><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
+    else if (mode == SRC_DECIM) train_wgrad_kernel<15, SRC_DECIM><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
+    else train_wgrad_kernel<5, SRC_UPCAT><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
 }
 
 struct Shape { int cin, cout, k, L, mode, cin0, cin1; };
@@ -595,6 +591,37 @@ bool train_naive()
 }  // namespace
 
 const char *train_error() { return g_train_err; }
+
+// CTA = 16 co x 64 ci; tiles of min(L, 128) positions of one frame, split over gridDim.z
+WgradGrid wgrad_grid_fp32(int B, int L, int Cin, int Cout)
+{
+    const int lt = std::min(L, 128);
+    const int nco = (Cout + 15) / 16, nci = (Cin + 63) / 64;
+    const int ntiles = B * ((L + lt - 1) / lt);
+    const int slices = std::max(1, std::min(ntiles, 1184 / (nco * nci)));           // ~4 blocks per SM over the grid
+    return WgradGrid{dim3((unsigned)nco, (unsigned)nci, (unsigned)slices), ntiles, lt};
+}
+
+int train_debug_layout(int n, int ci, int B, int T, int prec, int block, long long *f, int capacity)
+{
+    if (block < 0 || block > 2 * n) return train_fail("layout query: block %d outside 0 .. %d", block, 2 * n);
+    if (!f || capacity < kTrainLayoutFields) return train_fail("layout query: needs room for %d fields", kTrainLayoutFields);
+    std::vector<Shape> sh;
+    shapes_of(n, ci, T, sh);
+    Layout lo;
+    layout_of(sh, B, lo, prec);
+    const Shape &s = sh[block];
+    const bool tc = on_tc(prec, block);
+    const WgradGrid g = tc ? wgrad_grid_bf16(B, s.L, s.cin, s.cout, s.k) : wgrad_grid_fp32(B, s.L, s.cin, s.cout);
+    const long long b = sizeof(float), gz = g.grid.z;
+    const long long v[kTrainLayoutFields] = {
+        (long long)lo.z[block] * b, (long long)lo.act[block] * b, (long long)lo.ga[block] * b, (long long)lo.mean[block] * b,
+        (long long)lo.invstd[block] * b, (long long)lo.s1[block] * b, (long long)lo.s2[block] * b,
+        s.cin, s.cin0, s.cin1, s.cout, s.L, s.k, s.mode,
+        tc ? 1 : 0, g.grid.x, g.grid.y, gz, g.items, g.positions, (g.items + gz - 1) / gz, (long long)lo.total * b};
+    for (int i = 0; i < kTrainLayoutFields; ++i) f[i] = v[i];
+    return 0;
+}
 
 size_t train_workspace_bytes(int n, int ci, int B, int T, int prec)
 {

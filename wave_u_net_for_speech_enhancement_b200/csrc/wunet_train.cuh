@@ -49,5 +49,9 @@ int train_backward(int n_layers, int ci, const float *x, const float *y, const f
 // sum dz * in. `in` is built from src0 / src1 per `mode` as in the forward (ConvArgs). Synchronous.
 int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int Cin0, int Cin1, int Cout, const float *src0,
                      const float *src1, const float *w, const float *dz, float *out);
+// Host-only: where block `block`'s tensors live in the training workspace and how its weight gradient is launched
+// (the fields of wunet_debug_train_layout, include/wunet_b200.h).
+constexpr int kTrainLayoutFields = 22;
+int train_debug_layout(int n_layers, int ci, int B, int T, int prec, int block, long long *fields, int capacity);
 
 }  // namespace wunet

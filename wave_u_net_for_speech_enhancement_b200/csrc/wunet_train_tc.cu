@@ -231,17 +231,22 @@ int launch_wgrad_tc(const ConvArgs &a, const float *dz, float *dw, cudaStream_t 
 {
     constexpr int XROWS = (kWgPos + KS - 1 + 7) / 8 * 8;
     constexpr int smem = (kWgPos + XROWS) * 128 + 1024;
-    const int ntg = KS / kTapGroup, nco = (a.Cout + 63) / 64, nci = (a.Cin + 63) / 64;
-    const int cpf = (a.L + kWgPos - 1) / kWgPos;
-    const int items = a.B * cpf;
-    const int base = nco * ntg * nci;
-    const int slices = std::max(1, std::min(items, (2 * 132 + base - 1) / base));           // about two CTAs per SM
-    const dim3 grid((unsigned)(nco * ntg), (unsigned)nci, (unsigned)slices);
-    train_wgrad_tc_kernel<KS, MODE><<<grid, 128, smem, st>>>(a, dz, dw, cpf);
+    const WgradGrid g = wgrad_grid_bf16(a.B, a.L, a.Cin, a.Cout, KS);
+    train_wgrad_tc_kernel<KS, MODE><<<g.grid, 128, smem, st>>>(a, dz, dw, (a.L + kWgPos - 1) / kWgPos);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
 }  // namespace
+
+// CTA = 64 co x 5 taps x 64 ci; the (frame, 64-position chunk) items are split over gridDim.z
+WgradGrid wgrad_grid_bf16(int B, int L, int Cin, int Cout, int ksize)
+{
+    const int ntg = ksize / kTapGroup, nco = (Cout + 63) / 64, nci = (Cin + 63) / 64;
+    const int items = B * ((L + kWgPos - 1) / kWgPos);
+    const int base = nco * ntg * nci;
+    const int slices = std::max(1, std::min(items, (2 * 132 + base - 1) / base));           // about two CTAs per SM
+    return WgradGrid{dim3((unsigned)(nco * ntg), (unsigned)nci, (unsigned)slices), items, kWgPos};
+}
 
 size_t train_tc_packed_elems(int cout, int cin, int k) { return (size_t)((cin + 63) / 64) * k * cols_of(cout).npad * 64; }
 

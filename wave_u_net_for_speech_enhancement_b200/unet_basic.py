@@ -397,6 +397,12 @@ class Model(nn.Module):
         running statistics and leaves them and ``num_batches_tracked`` untouched (.eval()). fp32 or, with
         ``train_precision="bf16"``, bf16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
+        B, _, T = x.shape
+        if not frozen_bn and B * (T >> self.n_layers) == 1:
+            # torch.nn.BatchNorm1d in training mode refuses batch statistics of one value per channel (here: the middle
+            # block of a single frame of 2^n_layers samples); the reference raises this from self.middle
+            raise ValueError("Expected more than 1 value per channel when training, got input size "
+                             f"{torch.Size([B, self.n_layers * self.channels_interval, T >> self.n_layers])}")
         if not x.is_cuda:
             raise RuntimeError("wave_u_net_for_speech_enhancement_b200 has no CPU fallback: move the model and the "
                                "input to a CUDA (sm_90a) device")
