@@ -3,8 +3,9 @@
     WUNET_TC_TRACE=1 python -m wave_u_net_for_speech_enhancement_b200.build --force   # then move the .so aside
     WUNET_LIB_PATH=.../libwunet_b200_trace.so python tools/trace_levels.py 23 22 2> trace.txt
 
-Roles: 0 = TMA producer, 1 = MMA issuer (tile start / accumulator free / per stage), 2 = epilogue warp 0 (tile start /
-accumulator full), 3 = first MMA of every tap, 4 = upsample producer thread 0 (before / after the stage wait, after emit).
+Roles: 0 = TMA producer (around its operand-stage waits, after each weight-stage wait), 1 = consumer thread 0 (before / after
+each operand-stage wait), 2 = consumer thread 0 at the start of each epilogue, 4 = upsample producer thread 0 (before / after
+the stage wait, after the hand-off). Times are clock64 cycles from role 1's first stamp.
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -135,21 +135,40 @@ __device__ __forceinline__ void wgmma_batch(float (&acc)[MB][ACC], uint32_t a_lo
             wgmma_m64nNk16<16 * NT>(*reinterpret_cast<float (*)[8 * NT]>(&acc[mb][0]), a_lo + (uint32_t)(mb * 512 + 2 * k),
                                     b_lo + (uint32_t)(2 * k), hi);
 }
-// wgmma_batch for run-time nt = columns / 16 (1 .. ACC / 8) and nk (1 .. 4): one fence, the batch, one commit (one wgmma group).
-// The dispatch branches lie outside the fence ... commit region.
-template <int MB, int ACC, int NT = ACC / 8>
-__device__ __forceinline__ void wgmma_group(int nt, int nk, float (&acc)[MB][ACC], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+// NTAP consecutive taps of wgmma_batch: tap t reads the A rows one 128-byte row further down (+8 in descriptor units) and the
+// weight tile b_step (descriptor units) further on, in the same order as NTAP separate batches.
+template <int NT, int NK, int NTAP, int MB, int ACC>
+__device__ __forceinline__ void wgmma_batch_taps(float (&acc)[MB][ACC], uint32_t a_lo, uint32_t b_lo, uint32_t b_step, uint32_t hi)
+{
+#pragma unroll
+    for (int t = 0; t < NTAP; ++t) wgmma_batch<NT, NK>(acc, a_lo + (uint32_t)t * 8u, b_lo + (uint32_t)t * b_step, hi);
+}
+// wgmma_batch_taps for run-time nt = columns / 16 (1 .. ACC / 8) and nk (1 .. 4): one fence, the batch, one commit (one wgmma
+// group). The dispatch branches lie outside the fence ... commit region.
+template <int MB, int ACC, int NTAP = 1, int NT = ACC / 8>
+__device__ __forceinline__ void wgmma_group(int nt, int nk, float (&acc)[MB][ACC], uint32_t a_lo, uint32_t b_lo, uint32_t hi,
+                                            uint32_t b_step = 0)
 {
     if (NT == 1 || nt == NT) {
         switch (nk) {
-        case 1: wgmma_fence(); wgmma_batch<NT, 1>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
-        case 2: wgmma_fence(); wgmma_batch<NT, 2>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
-        case 3: wgmma_fence(); wgmma_batch<NT, 3>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
-        default: wgmma_fence(); wgmma_batch<NT, 4>(acc, a_lo, b_lo, hi); wgmma_commit(); break;
+        case 1: wgmma_fence(); wgmma_batch_taps<NT, 1, NTAP>(acc, a_lo, b_lo, b_step, hi); wgmma_commit(); break;
+        case 2: wgmma_fence(); wgmma_batch_taps<NT, 2, NTAP>(acc, a_lo, b_lo, b_step, hi); wgmma_commit(); break;
+        case 3: wgmma_fence(); wgmma_batch_taps<NT, 3, NTAP>(acc, a_lo, b_lo, b_step, hi); wgmma_commit(); break;
+        default: wgmma_fence(); wgmma_batch_taps<NT, 4, NTAP>(acc, a_lo, b_lo, b_step, hi); wgmma_commit(); break;
         }
     } else if constexpr (NT > 1) {
-        wgmma_group<MB, ACC, NT - 1>(nt, nk, acc, a_lo, b_lo, hi);
+        wgmma_group<MB, ACC, NTAP, NT - 1>(nt, nk, acc, a_lo, b_lo, hi, b_step);
     }
+}
+// wgmma_group for run-time ntap (1 .. NTAP) consecutive taps. Each wgmma group costs a fixed few hundred cycles on top of its
+// MMAs (per-role trace, H100), which dominated the narrow decoder blocks when every tap was a group of its own.
+constexpr int kMaxGroupTaps = 5;
+template <int MB, int ACC, int NTAP = kMaxGroupTaps>
+__device__ __forceinline__ void wgmma_group_taps(int ntap, int nt, int nk, float (&acc)[MB][ACC], uint32_t a_lo, uint32_t b_lo,
+                                                 uint32_t hi, uint32_t b_step)
+{
+    if (NTAP == 1 || ntap == NTAP) wgmma_group<MB, ACC, NTAP>(nt, nk, acc, a_lo, b_lo, hi, b_step);
+    else if constexpr (NTAP > 1) wgmma_group_taps<MB, ACC, NTAP - 1>(ntap, nt, nk, acc, a_lo, b_lo, hi, b_step);
 }
 __device__ __forceinline__ void st_shared_v4_if(uint32_t addr, const uint4 &v, bool pred)
 {
@@ -218,8 +237,8 @@ struct TcParams {
     long long *trace;          // WUNET_TC_TRACE builds: per-role clock64 stamps of CTA 0 (development)
     // merged tail chunk (MG = 1 instantiations): the last K chunk of a decoder block is [skip tail (TMA) | upsampled tail
     // (producers)] in ONE stage - one K chunk fewer for dec6 / dec9 / dec10 of the reference architecture
-    int pf_late;               // 1: the producers' register prefetch of their next unit is issued when the K loop reaches that unit (after the
-                               // TMA chunks in between have been handed on) instead of right after the previous unit's hand-off
+    int pf_late;               // 1 (default): the producers' register prefetch of their next unit is issued when the K loop reaches that unit
+                               // (after the TMA chunks in between have been handed on); 0: right after the previous unit's hand-off
     int split;                 // split-precision mode (SP kernels): activations are stored as [hi | lo] bf16 channel halves (2 C channels per
                                // row), the K loop runs [hi data x w_hi | lo data x w_hi | hi data x w_lo] and the epilogue stores hi and lo
     int mg;                    // 1: chunk_map's last entry (0x40) is such a merged chunk
@@ -508,6 +527,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // descriptor words: hi = SBO(1024 B) | SWIZZLE_128B, lo = (addr >> 4) | LBO(1)
         const uint32_t hi = (uint32_t)(1024 >> 4) | (1u << 30);
         int sa = 0, pa = 0, sb = 0, pb = 0;
+        int tr1 = 0, tr2 = 0; (void)tr1; (void)tr2;
         if (p.resident) mbar_wait(b_full, 0);
         for (int tile = first_tile; tile < total_tiles; tile += gridDim.x) {
             int b0, l0, n0;
@@ -521,7 +541,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int c = 0; c < p.nchunks; ++c) {
                 const ChunkInfo mci = chunk_info<UPCAT, MG, SP>(p, c);
                 const int nk = mci.nk;
+                if (threadIdx.x == 0) TRACE(1, tr1);
                 if (!(SP != 0 && mci.reuse)) mbar_wait(a_full + 8 * sa, pa);
+                if (threadIdx.x == 0) TRACE(1, tr1);
                 const uint32_t a_base = base + sm.a + sa * p.a_stage_bytes + (uint32_t)(wg * MB * 64 * 128);
                 const uint32_t a_lo0 = ((a_base >> 4) & 0x3FFFu) | (1u << 16);
                 for (int g = 0; g < p.ngroups; ++g) {
@@ -534,13 +556,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     }
                     const uint32_t b_lo0 = ((b_base >> 4) & 0x3FFFu) | (1u << 16);
                     const int t0 = g * p.tg, t_end = min(KS, (g + 1) * p.tg);
-                    // one wgmma group per tap: nk K16 steps x MB row blocks, each as wide as the CTA's columns. The stage is
-                    // released once all of them have completed. (Releasing it one group late, after a wgmma.wait_group 1 behind the
-                    // next stage's first group, measured about 5 % slower end to end on an H100 at 400 W.)
+                    // one wgmma group per run of up to kMaxGroupTaps taps (a whole decoder stage): per tap nk K16 steps x MB row
+                    // blocks, each as wide as the CTA's columns, in the order of one group per tap. The stage is released once all
+                    // of them have completed. (Releasing it one group late, after a wgmma.wait_group 1 behind the next stage's first
+                    // group, measured about 5 % slower end to end on an H100 at 400 W.)
 #pragma unroll 1
-                    for (int t = t0; t < t_end; ++t)
-                        wgmma_group(nt, nk, acc, a_lo0 + (uint32_t)t * 8u,               // tap shift: +128 B
-                                    b_lo0 + (uint32_t)(t - t0) * b_step, hi);
+                    for (int t = t0; t < t_end; t += kMaxGroupTaps)
+                        wgmma_group_taps<MB, 8 * NB>(min(kMaxGroupTaps, t_end - t), nt, nk, acc, a_lo0 + (uint32_t)t * 8u,   // tap shift: +128 B
+                                                     b_lo0 + (uint32_t)(t - t0) * b_step, hi, b_step);
                     wgmma_wait0();
                     if (!p.resident) {
                         if (wg_leader) mbar_arrive(b_empty + 8 * sb);
@@ -554,6 +577,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
             // epilogue
+            if (threadIdx.x == 0) TRACE(2, tr2);
 #pragma unroll
             for (int mb = 0; mb < MB; ++mb) {
 #pragma unroll
@@ -1694,7 +1718,8 @@ struct TcState {
     bool attr_set = false;
     bool pdl = false;                  // programmatic dependent launch between the blocks (WUNET_TC_PDL=1); measured slower, off
     bool merge = true;                 // merged tail chunks (WUNET_TC_MERGE=0 switches them off for A/B measurements)
-    bool pf_late = false;              // WUNET_TC_PFLATE=1: see TcParams::pf_late
+    bool pf_late = true;               // see TcParams::pf_late; WUNET_TC_PFLATE=0 switches it off (A/B measurements, tests). Since the
+                                       // taps of a stage share one wgmma group, the late prefetch is the faster one (dec4 ... dec10, H100)
     bool gemm = true;                  // dense GEMM over frames for blocks of at most 16 samples (WUNET_TC_GEMM=0 switches it off)
     // row-pair mode (WUNET_TC_PAIR bit 0: first tensor-core encoder block, bit 1: last decoder block + head): virtual blocks with
     // doubled channel counts and Toeplitz-expanded weights (pair_weight), planned on frames of half the length
@@ -1797,7 +1822,7 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         const char *pe = getenv("WUNET_TC_PDL");
         st->pdl = pe && pe[0] == '1';
         if (const char *xe = getenv("WUNET_TC_MERGE")) st->merge = xe[0] != '0';
-        if (const char *xe = getenv("WUNET_TC_PFLATE")) st->pf_late = xe[0] == '1';
+        if (const char *xe = getenv("WUNET_TC_PFLATE")) st->pf_late = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_GEMM")) st->gemm = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_L2PROMO")) st->enc_l2promo = atoi(xe);
         if (const char *xe = getenv("WUNET_TC_PAIR")) st->pair_mask = atoi(xe) & 3;
