@@ -217,6 +217,7 @@ int wunet_train_backward_part_prec(wunet_ctx *ctx, const float *x, const float *
  * a learnable front end, an adversarial perturbation), and eval-mode BatchNorm for fine-tuning with frozen statistics. */
 #define WUNET_TRAIN_FROZEN_BN      1  /* BatchNorm uses (and never updates) the running statistics: eval-mode BN */
 #define WUNET_TRAIN_NO_PARAM_GRADS 2  /* backward: no parameter gradients (g_* may be NULL), only dx */
+#define WUNET_TRAIN_DETERMINISTIC 16  /* bitwise repeatable step: no float atomics; the workspace grows (see below) */
 /* wunet_train_forward_ex: with WUNET_TRAIN_FROZEN_BN, BatchNorm normalises by bn_running_mean / bn_running_var, which are only
  *   read (momentum is unused): model/unet_basic.py in .eval() mode, with the activations kept for the backward. The forward
  *   ignores WUNET_TRAIN_NO_PARAM_GRADS. The workspace size is wunet_train_workspace_bytes_prec (frozen mode needs nothing extra).
@@ -225,9 +226,20 @@ int wunet_train_backward_part_prec(wunet_ctx *ctx, const float *x, const float *
  * wunet_train_backward_ex: dx [B][1][T] (device, or NULL) is fully overwritten with the gradient of x. It belongs to part 1
  *   (block 0 is there): pass it with part -1 or 1; dx with part 0 is WUNET_EINVAL. With WUNET_TRAIN_NO_PARAM_GRADS no weight
  *   gradient, bias or BatchNorm-parameter reduction runs and nothing is written through g_*.
- * The backward must use the precision, the workspace and the WUNET_TRAIN_FROZEN_BN bit of its forward.
- * Unknown flag bits -> WUNET_EINVAL. Call sites: loss.backward() through model(x) with x.requires_grad in .train() mode, and
- * through model(x) in .eval() mode (trainer/trainer.py:35-37 with model.eval()). */
+ * WUNET_TRAIN_DETERMINISTIC: the weight gradients and the head's gradients combine their partial sums in an order that depends
+ *   only on (n_layers, channels_interval, B, T, precision): each slice of a weight-gradient grid stores its partial dW to a
+ *   scratch region after the activations, and one kernel adds the slices in index order (in double); the head's per-CTA
+ *   partials are summed likewise. Every other reduction of the step already has a fixed order, so y, the running buffers, all
+ *   parameter gradients and dx are bitwise repeatable for the same inputs on the same GPU model, whatever the workspace held
+ *   before. The workspace must hold wunet_train_workspace_bytes_ex with this bit. Without it nothing changes. With the
+ *   environment variable WUNET_TRAIN_NAIVE=1 (the naive cross-check kernels) a backward with parameter gradients under this
+ *   flag is WUNET_ECUDA. Call site: trainer/base_trainer.py:140-143 (torch.backends.cudnn.deterministic = True).
+ * The backward must use the precision, the workspace and the WUNET_TRAIN_FROZEN_BN and WUNET_TRAIN_DETERMINISTIC bits of its
+ * forward. Bits other than 1, 2 and 16 -> WUNET_EINVAL. Call sites: loss.backward() through model(x) with x.requires_grad in
+ * .train() mode, and through model(x) in .eval() mode (trainer/trainer.py:35-37 with model.eval()). */
+/* Bytes of training workspace for these flags: wunet_train_workspace_bytes_prec, plus the deterministic scratch when flags has
+ * WUNET_TRAIN_DETERMINISTIC. 0 on error (unknown flag bits included). */
+size_t wunet_train_workspace_bytes_ex(const wunet_ctx *ctx, int B, int T, int precision, int flags);
 int wunet_train_forward_ex(wunet_ctx *ctx, const float *x, float *y, int B, int T, const float *const *conv_w,
                            const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
                            float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,

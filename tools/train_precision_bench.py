@@ -1,7 +1,9 @@
-"""Training-step time of the reference architecture (n_layers 12, channels_interval 24, T = 16384) in three legs:
+"""Training-step time of the reference architecture (n_layers 12, channels_interval 24, T = 16384) in five legs:
 
     native fp32   Model(train_backend="native", train_precision="fp32")   fp32 FFMA convolutions (wunet_train.cu)
     native bf16   Model(train_backend="native", train_precision="bf16")   bf16 wgmma convolutions (wunet_train_tc.cu)
+    *_det         the same two under torch.backends.cudnn.deterministic = True: deterministic mode (ordered weight- and
+                  head-gradient sums instead of float atomics)
     autocast      Model(train_backend="torch") under torch.autocast("cuda", torch.bfloat16): PyTorch eager + cuDNN
 
 Each step is what trainer/trainer.py:34-38 does: forward, MSE loss, backward, Adam (lr 1e-3; train.py:31-35). Per batch size
@@ -28,7 +30,9 @@ from wave_u_net_for_speech_enhancement_b200 import Model  # noqa: E402
 
 LEGS = {
     "native_fp32": dict(train_backend="native", train_precision="fp32"),
+    "native_fp32_det": dict(train_backend="native", train_precision="fp32"),
     "native_bf16": dict(train_backend="native", train_precision="bf16"),
+    "native_bf16_det": dict(train_backend="native", train_precision="bf16"),
     "autocast_bf16": dict(train_backend="torch"),
 }
 
@@ -60,6 +64,8 @@ def run_steps(leg, state, n, timed):
     crit = torch.nn.MSELoss()
     ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(n)]
     losses = []
+    saved = torch.backends.cudnn.deterministic
+    torch.backends.cudnn.deterministic = leg.endswith("_det")
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for i in range(n):
@@ -77,6 +83,7 @@ def run_steps(leg, state, n, timed):
         losses.append(loss.detach())
     torch.cuda.synchronize()
     wall = time.perf_counter() - t0
+    torch.backends.cudnn.deterministic = saved
     if not timed:
         return None
     ph = np.array([[e[0].elapsed_time(e[1]), e[1].elapsed_time(e[2]), e[2].elapsed_time(e[3])] for e in ev])

@@ -14,6 +14,7 @@ PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC}
 
 TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mode BatchNorm
 TRAIN_NO_PARAM_GRADS = 2   # backward: input gradient only
+TRAIN_DETERMINISTIC = 16   # bitwise repeatable step (no float atomics; larger workspace)
 
 _lib = None
 
@@ -68,6 +69,8 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_backward_part.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, cs, vp, ci]
     lib.wunet_train_workspace_bytes_prec.argtypes = [vp, ci, ci, ci]
     lib.wunet_train_workspace_bytes_prec.restype = cs
+    lib.wunet_train_workspace_bytes_ex.argtypes = [vp, ci, ci, ci, ci]
+    lib.wunet_train_workspace_bytes_ex.restype = cs
     lib.wunet_train_forward_prec.argtypes = lib.wunet_train_forward.argtypes + [ci]
     lib.wunet_train_backward_part_prec.argtypes = lib.wunet_train_backward_part.argtypes + [ci]
     lib.wunet_train_forward_ex.argtypes = lib.wunet_train_forward_prec.argtypes + [ci]
@@ -90,7 +93,7 @@ EXPORTED_SYMBOLS = [
     "wunet_debug_pair_weights",
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
-    "wunet_train_forward_ex", "wunet_train_backward_ex", "wunet_debug_train_layout",
+    "wunet_train_forward_ex", "wunet_train_backward_ex", "wunet_train_workspace_bytes_ex", "wunet_debug_train_layout",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]

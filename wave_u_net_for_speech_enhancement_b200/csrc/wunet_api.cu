@@ -479,6 +479,27 @@ size_t wunet_train_workspace_bytes_prec(const wunet_ctx *c, int B, int T, int pr
     return train_workspace_bytes(c->n, c->ci, B, T, prec);
 }
 
+static const int kTrainFlags = WUNET_TRAIN_FROZEN_BN | WUNET_TRAIN_NO_PARAM_GRADS | WUNET_TRAIN_DETERMINISTIC;
+
+// the flags the training kernels act on (TrainFlags) for the public bits
+static int train_flags(int flags)
+{
+    return ((flags & WUNET_TRAIN_FROZEN_BN) ? TRAIN_FROZEN_BN : 0) | ((flags & WUNET_TRAIN_NO_PARAM_GRADS) ? TRAIN_NO_PARAM_GRADS : 0) |
+           ((flags & WUNET_TRAIN_DETERMINISTIC) ? TRAIN_DETERMINISTIC : 0);
+}
+
+size_t wunet_train_workspace_bytes_ex(const wunet_ctx *c, int B, int T, int precision, int flags)
+{
+    if (check_shape(c, B, T) != WUNET_OK) return 0;
+    const int prec = train_prec(precision);
+    if (prec < 0) return 0;
+    if (flags & ~kTrainFlags) {
+        fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
+        return 0;
+    }
+    return train_workspace_bytes(c->n, c->ci, B, T, prec, train_flags(flags));
+}
+
 int wunet_train_forward(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
                         const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
                         float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
@@ -497,8 +518,6 @@ int wunet_train_forward_prec(wunet_ctx *c, const float *x, float *y, int B, int 
                                   out_b, momentum, workspace, workspace_bytes, stream, precision, 0);
 }
 
-static const int kTrainFlags = WUNET_TRAIN_FROZEN_BN | WUNET_TRAIN_NO_PARAM_GRADS;
-
 int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
                            const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
                            float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
@@ -516,11 +535,11 @@ int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T,
                                   "middle block)", T);
     if (!x || !y || !workspace || !conv_w || !conv_b || !bn_weight || !bn_bias || !bn_running_mean || !bn_running_var || !out_w || !out_b)
         return fail(WUNET_EINVAL, "null argument");
-    const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
+    const int tflags = train_flags(flags & ~WUNET_TRAIN_NO_PARAM_GRADS);               // NO_PARAM_GRADS: nothing to do here
+    const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec, tflags);
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b};
-    const int tflags = (flags & WUNET_TRAIN_FROZEN_BN) ? TRAIN_FROZEN_BN : 0;        // NO_PARAM_GRADS: nothing to do here
     if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec, tflags))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
@@ -571,12 +590,12 @@ int wunet_train_backward_ex(wunet_ctx *c, const float *x, const float *y, const 
     if (!x || !y || !dy || !workspace || !conv_w || !bn_weight || !bn_bias || !out_w ||
         (pgrads && (!g_conv_w || !g_conv_b || !g_bn_weight || !g_bn_bias || !g_out_w || !g_out_b)))
         return fail(WUNET_EINVAL, "null argument");
-    const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec);
+    const int tflags = train_flags(flags);
+    const size_t need = train_workspace_bytes(c->n, c->ci, B, T, prec, tflags);
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, nullptr, bn_weight, bn_bias, nullptr, nullptr, out_w, nullptr};
     const TrainGrads G{g_conv_w, g_conv_b, g_bn_weight, g_bn_bias, g_out_w, g_out_b};
-    const int tflags = ((flags & WUNET_TRAIN_FROZEN_BN) ? TRAIN_FROZEN_BN : 0) | (pgrads ? 0 : TRAIN_NO_PARAM_GRADS);
     if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec, dx, tflags))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;

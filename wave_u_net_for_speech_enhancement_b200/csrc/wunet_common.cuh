@@ -78,8 +78,9 @@ int launch_pack_fp32(const float *w, const float *bias, const float *g, const fl
 // launch_conv_bf16: launch_conv_fp32's operator with a.wp pointing at the bf16 forward (or input-gradient) packing written by
 // train_tc_pack; ksize 15 (DIRECT, DECIM) or 5 (DIRECT, UPCAT).
 int launch_conv_bf16(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
-// dw[co][ci][k] += sum_{b,l} dz[b][co][l] * in(b, ci, l + k - pad), in read through `a` as the forward reads it (dw zeroed first)
-int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st);
+// dw[co][ci][k] += sum_{b,l} dz[b][co][l] * in(b, ci, l + k - pad), in read through `a` as the forward reads it (dw zeroed first).
+// slices = true: slice z of the grid stores its partial sums to dw + z * Cout * Cin * K instead (nothing zeroed first)
+int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices = false);
 // Launch geometry of the two weight-gradient kernels, the one definition their launchers and wunet_debug_train_layout use:
 // grid, number of (frame, position tile) work items that gridDim.z slices share, and positions per item.
 struct WgradGrid { dim3 grid; int items, positions; };

@@ -6,6 +6,9 @@
 //                                       flipped, read from dz (train_pack_kernel writes both packings every step);
 //   weight gradient                  -> train_wgrad_kernel below (register-tiled reduction over (batch, position) tiles staged in
 //                                       shared memory, split over the batch, combined with atomicAdd).
+// TRAIN_DETERMINISTIC replaces the two float-atomic combines (weight gradients, head gradients) with partial sums stored to a
+// scratch region after the workspace layout and summed in an order fixed by the shapes (train_slice_sum_kernel,
+// train_head_sum_kernel); every other reduction of the step already has a fixed order.
 // The naive one-thread-per-output kernels they replace are kept as WUNET_TRAIN_NAIVE=1 (cross-check, tests).
 // TRAIN_BF16 (Model(train_precision="bf16")): the forward conv, input gradient and weight gradient of every block but the
 // first (Cin = 1) run on the bf16 tensor-core kernels of wunet_train_tc.cu instead; everything else is the same fp32 code.
@@ -147,12 +150,33 @@ __global__ void train_bn_act_kernel(const float *__restrict__ z, const float *__
 // ---------------------------------------------------------------------------------------------
 // head: y = tanh(sum_c Wo[c] cat[c] + bo), cat = [a_last (C channels) | x]   (model/unet_basic.py:98-99)
 //   dpre = dy (1 - y^2);  dWo[c] = sum dpre cat[c];  dbo = sum dpre;  d a_last[c] = Wo[c] dpre
-// g_wo == nullptr (TRAIN_NO_PARAM_GRADS): d a_last only
+// g_wo == nullptr (TRAIN_NO_PARAM_GRADS): d a_last only. The warp sums of dWo and dbo are combined with atomicAdd or, with
+// PARTIALS (deterministic mode), summed in warp order per CTA in double and stored to part[blockIdx.x][C + 2] (dWo, dbo) for
+// train_head_sum_kernel.
+template <bool PARTIALS>
 __global__ void __launch_bounds__(256) train_head_bwd_kernel(const float *__restrict__ dy, const float *__restrict__ y,
                                                              const float *__restrict__ a_last, const float *__restrict__ x,
                                                              const float *__restrict__ wo, float *__restrict__ ga_last,
-                                                             float *__restrict__ g_wo, float *__restrict__ g_bo, int B, int C, int T)
+                                                             float *__restrict__ g_wo, float *__restrict__ g_bo,
+                                                             double *__restrict__ part, int B, int C, int T)
 {
+    __shared__ double sh[8];
+    // warp sum of v -> g[c] (atomically) or -> part (CTA sum in warp order); every thread of the CTA calls it
+    auto combine = [&](float v, float *g, int c) {
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (!PARTIALS) {
+            if ((threadIdx.x & 31) == 0) atomicAdd(g, v);
+            return;
+        }
+        if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = (double)v;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double s = 0.0;
+            for (int w = 0; w < 8; ++w) s += sh[w];
+            part[(size_t)blockIdx.x * (C + 2) + c] = s;
+        }
+        __syncthreads();
+    };
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;      // over [B][T]
     const bool ok = i < (long long)B * T;
     const int b = ok ? (int)(i / T) : 0, l = ok ? (int)(i - (long long)b * T) : 0;
@@ -172,12 +196,35 @@ __global__ void __launch_bounds__(256) train_head_bwd_kernel(const float *__rest
         } else {
             v = ok ? dpre * x[i] : 0.f;
         }
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if ((threadIdx.x & 31) == 0) atomicAdd(g_wo + c, v);
+        combine(v, g_wo + c, c);
     }
-    float v = dpre;
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(g_bo, v);
+    combine(dpre, g_bo, C + 1);
+}
+
+// deterministic head gradients: out c (0 .. C: dWo[c], C + 1: dbo) = blockIdx.x of this kernel, the sum of the nparts CTA
+// partials of train_head_bwd_kernel<true> in double, in a fixed order (strided per thread, then block_sum)
+__global__ void __launch_bounds__(256) train_head_sum_kernel(const double *__restrict__ part, int nparts, int C,
+                                                             float *__restrict__ g_wo, float *__restrict__ g_bo)
+{
+    __shared__ double sh[8];
+    const int c = blockIdx.x;
+    double s = 0.0;
+    for (int j = threadIdx.x; j < nparts; j += blockDim.x) s += part[(size_t)j * (C + 2) + c];
+    const double t = block_sum(s, sh);
+    if (threadIdx.x == 0) {
+        if (c <= C) g_wo[c] = (float)t;
+        else *g_bo = (float)t;
+    }
+}
+
+// deterministic weight gradients: dw[i] = sum over the slices z = 0, 1, ... of part[z * n + i], in that order, in double
+__global__ void train_slice_sum_kernel(const float *__restrict__ part, float *__restrict__ dw, int slices, long long n)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    double s = 0.0;
+    for (int z = 0; z < slices; ++z) s += (double)part[(size_t)z * n + i];
+    dw[i] = (float)s;
 }
 
 // BatchNorm + LeakyReLU backward, reductions of channel c = blockIdx.x:
@@ -280,7 +327,7 @@ __global__ void __launch_bounds__(128) train_conv_bwd_data_kernel(const float *_
 }
 
 // dW[co][ci][k] = sum_b sum_l dz[b][co][l] * in(b, ci, l + k - pad).  Block = (co, group of 4 ci, slice of the batch);
-// the slices are combined with atomicAdd (dW is zeroed first).
+// the slices are combined with atomicAdd (dW is zeroed first); there is no deterministic form (TRAIN_DETERMINISTIC refuses it).
 template <int KS, int MODE>
 __global__ void __launch_bounds__(128) train_conv_bwd_weight_kernel(const ConvArgs a, const float *__restrict__ dz, float *__restrict__ dw)
 {
@@ -440,8 +487,9 @@ __global__ void train_fill_kernel(float *__restrict__ p, float v, int n)
 // its lanes own ci = lane and lane + 32: conflict-free rows). The reduction runs over tiles of `lt` positions of one frame,
 // staged in shared memory (the block input is built on the fly by fetch_src: decimate / interpolate + cat), 4 positions per
 // inner step: 2 x (4 + KS - 1) + 8 shared loads for 16 KS FFMA. gridDim.z slices of the (frame, tile) list are combined
-// with atomicAdd (dW is zeroed first).
-template <int KS, int MODE>
+// with atomicAdd (dW is zeroed first) or, with SLICES (deterministic mode), each slice stores its partial sums to its own
+// copy of dW at dw + blockIdx.z * Cout Cin KS.
+template <int KS, int MODE, bool SLICES>
 __global__ void __launch_bounds__(256) train_wgrad_kernel(const ConvArgs a, const float *__restrict__ dz, float *__restrict__ dw, int lt)
 {
     constexpr int PAD = (KS - 1) / 2, CO_T = 16, CI_T = 64, LT_MAX = 128;
@@ -492,6 +540,7 @@ __global__ void __launch_bounds__(256) train_wgrad_kernel(const ConvArgs a, cons
                 }
         }
     }
+    if (SLICES) dw += (size_t)blockIdx.z * a.Cout * a.Cin * KS;
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -499,18 +548,30 @@ __global__ void __launch_bounds__(256) train_wgrad_kernel(const ConvArgs a, cons
             const int co = co0 + 2 * warp + i, ci = ci0 + lane + 32 * j;
             if (co < a.Cout && ci < a.Cin) {
 #pragma unroll
-                for (int k = 0; k < KS; ++k) atomicAdd(dw + ((size_t)co * a.Cin + ci) * KS + k, acc[i][j][k]);
+                for (int k = 0; k < KS; ++k) {
+                    float *d = dw + ((size_t)co * a.Cin + ci) * KS + k;
+                    if (SLICES) *d = acc[i][j][k];
+                    else atomicAdd(d, acc[i][j][k]);
+                }
             }
         }
 }
 
-// the tiled fp32 weight gradient (dw zeroed first); mode DIRECT / DECIM: 15 taps, UPCAT: 5
-void launch_wgrad_fp32(const ConvArgs &a, const float *dz, float *dw, int mode, cudaStream_t st)
+template <bool SLICES>
+void launch_wgrad_fp32_as(const ConvArgs &a, const float *dz, float *dw, int mode, cudaStream_t st)
 {
     const WgradGrid g = wgrad_grid_fp32(a.B, a.L, a.Cin, a.Cout);
-    if (mode == SRC_DIRECT) train_wgrad_kernel<15, SRC_DIRECT><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
-    else if (mode == SRC_DECIM) train_wgrad_kernel<15, SRC_DECIM><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
-    else train_wgrad_kernel<5, SRC_UPCAT><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
+    if (mode == SRC_DIRECT) train_wgrad_kernel<15, SRC_DIRECT, SLICES><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
+    else if (mode == SRC_DECIM) train_wgrad_kernel<15, SRC_DECIM, SLICES><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
+    else train_wgrad_kernel<5, SRC_UPCAT, SLICES><<<g.grid, 256, 0, st>>>(a, dz, dw, g.positions);
+}
+
+// the tiled fp32 weight gradient (dw zeroed first; with `slices`, the per-slice partial sums of train_wgrad_kernel<.., true>);
+// mode DIRECT / DECIM: 15 taps, UPCAT: 5
+void launch_wgrad_fp32(const ConvArgs &a, const float *dz, float *dw, int mode, cudaStream_t st, bool slices = false)
+{
+    if (slices) launch_wgrad_fp32_as<true>(a, dz, dw, mode, st);
+    else launch_wgrad_fp32_as<false>(a, dz, dw, mode, st);
 }
 
 struct Shape { int cin, cout, k, L, mode, cin0, cin1; };
@@ -581,6 +642,21 @@ ConvArgs conv_args(const std::vector<Shape> &sh, const Layout &lo, float *ws, co
 
 unsigned blocks_for(long long n, int per) { return (unsigned)((n + per - 1) / per); }
 
+// TRAIN_DETERMINISTIC scratch in floats, placed at lo.total: the larger of one block's per-slice weight-gradient partials
+// (gridDim.z copies of its dW; the grids depend on the shapes only) and the head's CTA partials (doubles). The blocks use it
+// one after another on the stream.
+size_t det_scratch_floats(const std::vector<Shape> &sh, int B, int T, int prec)
+{
+    const int last = (int)sh.size() - 1;
+    size_t m = 2 * (size_t)blocks_for((long long)B * T, 256) * (sh[last].cout + 2);
+    for (int i = 0; i <= last; ++i) {
+        const Shape &s = sh[i];
+        const WgradGrid g = on_tc(prec, i) ? wgrad_grid_bf16(B, s.L, s.cin, s.cout, s.k) : wgrad_grid_fp32(B, s.L, s.cin, s.cout);
+        m = std::max(m, (size_t)g.grid.z * s.cout * s.cin * s.k);
+    }
+    return m;
+}
+
 // WUNET_TRAIN_NAIVE=1: the one-thread-per-output reference kernels instead of the tuned ones (cross-check)
 bool train_naive()
 {
@@ -623,13 +699,14 @@ int train_debug_layout(int n, int ci, int B, int T, int prec, int block, long lo
     return 0;
 }
 
-size_t train_workspace_bytes(int n, int ci, int B, int T, int prec)
+size_t train_workspace_bytes(int n, int ci, int B, int T, int prec, int flags)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
     layout_of(sh, B, lo, prec);
-    return lo.total * sizeof(float);
+    const size_t scratch = (flags & TRAIN_DETERMINISTIC) ? det_scratch_floats(sh, B, T, prec) : 0;
+    return (lo.total + scratch) * sizeof(float);
 }
 
 int train_forward(int n, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum, void *workspace,
@@ -696,15 +773,26 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
     const int last = 2 * n, C = sh[last].cout;
     const bool naive = train_naive() && prec == TRAIN_FP32;
     const bool frozen = flags & TRAIN_FROZEN_BN, pgrads = !(flags & TRAIN_NO_PARAM_GRADS);
+    const bool det = pgrads && (flags & TRAIN_DETERMINISTIC);      // without parameter gradients nothing is summed atomically
+    float *scratch = ws + lo.total;                                 // TRAIN_DETERMINISTIC only (det_scratch_floats)
     if (part < -1 || part > 1) return train_fail("training backward: part must be -1, 0 or 1 (got %d)", part);
     if (dx && part == 0) return train_fail("training backward: dx is written by part 1 (or -1), not part 0");
+    if (det && naive) return train_fail("training backward: WUNET_TRAIN_NAIVE=1 has no deterministic weight gradient");
     if (part != 1) {
-        if (pgrads) {
-            cudaMemsetAsync(G.out_w, 0, (C + 1) * sizeof(float), st);
-            cudaMemsetAsync(G.out_b, 0, sizeof(float), st);
+        const unsigned hb = blocks_for((long long)B * T, 256);
+        if (det) {
+            double *hp = reinterpret_cast<double *>(scratch);
+            train_head_bwd_kernel<true><<<hb, 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last], G.out_w,
+                                                            G.out_b, hp, B, C, T);
+            train_head_sum_kernel<<<(unsigned)(C + 2), 256, 0, st>>>(hp, (int)hb, C, G.out_w, G.out_b);
+        } else {
+            if (pgrads) {
+                cudaMemsetAsync(G.out_w, 0, (C + 1) * sizeof(float), st);
+                cudaMemsetAsync(G.out_b, 0, sizeof(float), st);
+            }
+            train_head_bwd_kernel<false><<<hb, 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last],
+                                                             pgrads ? G.out_w : nullptr, G.out_b, nullptr, B, C, T);
         }
-        train_head_bwd_kernel<<<blocks_for((long long)B * T, 256), 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last],
-                                                                                 pgrads ? G.out_w : nullptr, G.out_b, B, C, T);
     }
     const int i_hi = (part == 1) ? n : last, i_lo = (part == 0) ? n + 1 : 0;
     for (int i = i_hi; i >= i_lo; --i) {
@@ -724,16 +812,23 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         const ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
         if (pgrads) {
             train_channel_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, G.conv_b[i], B, s.cout, s.L);
-            // weight gradient
-            cudaMemsetAsync(G.conv_w[i], 0, (size_t)s.cout * s.cin * s.k * sizeof(float), st);
+            // weight gradient: gridDim.z slices combined with atomicAdd into the zeroed dW or, in deterministic mode, stored to
+            // the scratch and summed in slice order
+            const long long nw = (long long)s.cout * s.cin * s.k;
+            float *wdst = det ? scratch : G.conv_w[i];
+            if (!det) cudaMemsetAsync(G.conv_w[i], 0, (size_t)nw * sizeof(float), st);
             const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
             if (on_tc(prec, i)) {
-                if (launch_wgrad_bf16(a, ga, G.conv_w[i], s.k, s.mode, st) < 0) return train_fail("training backward, block %d: bf16 weight-gradient launch failed", i);
+                if (launch_wgrad_bf16(a, ga, wdst, s.k, s.mode, st, det) < 0) return train_fail("training backward, block %d: bf16 weight-gradient launch failed", i);
             } else if (!naive) {
-                launch_wgrad_fp32(a, ga, G.conv_w[i], s.mode, st);
+                launch_wgrad_fp32(a, ga, wdst, s.mode, st, det);
             } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
             else if (s.mode == SRC_DECIM) train_conv_bwd_weight_kernel<15, SRC_DECIM><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
             else train_conv_bwd_weight_kernel<5, SRC_UPCAT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
+            if (det) {
+                const WgradGrid g = on_tc(prec, i) ? wgrad_grid_bf16(B, s.L, s.cin, s.cout, s.k) : wgrad_grid_fp32(B, s.L, s.cin, s.cout);
+                train_slice_sum_kernel<<<blocks_for(nw, 256), 256, 0, st>>>(scratch, G.conv_w[i], (int)g.grid.z, nw);
+            }
         }
         // input gradient and its routing to the producers of the block input
         if (s.mode != SRC_DIRECT) {

@@ -28,11 +28,14 @@ struct TrainGrads {
 enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1 };
 // TRAIN_FROZEN_BN: BatchNorm normalises by the running statistics and never updates them (eval-mode BatchNorm); the forward
 // and the backward of one step must agree on it. TRAIN_NO_PARAM_GRADS (backward only): no parameter gradient is computed
-// (G may hold null pointers), only the input gradient.
-enum TrainFlags : int { TRAIN_FROZEN_BN = 1, TRAIN_NO_PARAM_GRADS = 2 };
+// (G may hold null pointers), only the input gradient. TRAIN_DETERMINISTIC: the weight and head gradients combine their
+// partial sums in an order fixed by the shapes (slices stored to a scratch region after the workspace layout, then summed in
+// index order) instead of with float atomics; the workspace grows by that scratch, and the forward and the backward of one
+// step must agree on it.
+enum TrainFlags : int { TRAIN_FROZEN_BN = 1, TRAIN_NO_PARAM_GRADS = 2, TRAIN_DETERMINISTIC = 4 };
 
 const char *train_error();
-size_t train_workspace_bytes(int n_layers, int ci, int B, int T, int prec = TRAIN_FP32);
+size_t train_workspace_bytes(int n_layers, int ci, int B, int T, int prec = TRAIN_FP32, int flags = 0);
 // y = model(x) with BatchNorm in training mode (or, with TRAIN_FROZEN_BN, eval mode); keeps every pre-BN output and
 // activation in `workspace` for the backward
 int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum,

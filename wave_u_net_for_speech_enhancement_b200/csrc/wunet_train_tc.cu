@@ -17,7 +17,8 @@
 //                           [position][64 co] and the input as [position][64 ci] (128B-swizzled), and fed MN-major
 //                           (imm-trans = 1): a tap advances the B descriptor by one 128-byte row, exactly as in the forward. A
 //                           CTA owns 64 co x 64 ci x 5 taps (160 accumulator registers per thread); the (frame, 64-position)
-//                           chunks are split over gridDim.z and combined with fp32 atomicAdd.
+//                           chunks are split over gridDim.z and combined with fp32 atomicAdd or, in deterministic mode,
+//                           stored per slice and summed in slice order by wunet_train.cu.
 //
 // Tiles never straddle two frames: a tile's rows past the frame end are computed and discarded, and positions outside
 // [0, L) read as zero (Conv1d padding, per frame), so frames shorter than a tile (the bottom of the U) are padded, never packed.
@@ -118,7 +119,8 @@ __global__ void __launch_bounds__(256, 2) train_conv_tc_kernel(const ConvArgs a,
     }
 }
 
-template <int KS, int MODE>
+// SLICES (deterministic mode): slice blockIdx.z stores its partial sums to its own copy of dW at dw + blockIdx.z * Cout Cin KS
+template <int KS, int MODE, bool SLICES>
 __global__ void __launch_bounds__(128) train_wgrad_tc_kernel(const ConvArgs a, const float *__restrict__ dz, float *__restrict__ dw,
                                                              int chunks_per_frame)
 {
@@ -165,13 +167,18 @@ __global__ void __launch_bounds__(128) train_wgrad_tc_kernel(const ConvArgs a, c
         wgmma_wait0();
     }
     // fragment: row (co) = 16 wq + lane / 4 (+8), column (ci) = 2 (lane % 4) (+1) of every 8-column group
+    if (SLICES) dw += (size_t)blockIdx.z * a.Cout * a.Cin * KS;
 #pragma unroll
     for (int tt = 0; tt < kTapGroup; ++tt)
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
             const int co = co0 + 16 * wq + (lane >> 2) + 8 * ((j >> 1) & 1);
             const int ci = ci0 + 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
-            if (co < a.Cout && ci < a.Cin) atomicAdd(dw + ((size_t)co * a.Cin + ci) * KS + t0 + tt, acc[tt][j]);
+            if (co < a.Cout && ci < a.Cin) {
+                float *d = dw + ((size_t)co * a.Cin + ci) * KS + t0 + tt;
+                if (SLICES) *d = acc[tt][j];
+                else atomicAdd(d, acc[tt][j]);
+            }
         }
 }
 
@@ -227,12 +234,14 @@ int launch_conv_tc_nt(const ConvArgs &a, cudaStream_t st)
 }
 
 template <int KS, int MODE>
-int launch_wgrad_tc(const ConvArgs &a, const float *dz, float *dw, cudaStream_t st)
+int launch_wgrad_tc(const ConvArgs &a, const float *dz, float *dw, cudaStream_t st, bool slices)
 {
     constexpr int XROWS = (kWgPos + KS - 1 + 7) / 8 * 8;
     constexpr int smem = (kWgPos + XROWS) * 128 + 1024;
     const WgradGrid g = wgrad_grid_bf16(a.B, a.L, a.Cin, a.Cout, KS);
-    train_wgrad_tc_kernel<KS, MODE><<<g.grid, 128, smem, st>>>(a, dz, dw, (a.L + kWgPos - 1) / kWgPos);
+    const int cpf = (a.L + kWgPos - 1) / kWgPos;
+    if (slices) train_wgrad_tc_kernel<KS, MODE, true><<<g.grid, 128, smem, st>>>(a, dz, dw, cpf);
+    else train_wgrad_tc_kernel<KS, MODE, false><<<g.grid, 128, smem, st>>>(a, dz, dw, cpf);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -267,11 +276,11 @@ int launch_conv_bf16(const ConvArgs &a, int ksize, int mode, cudaStream_t st)
     return -1;
 }
 
-int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st)
+int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices)
 {
-    if (ksize == 15 && mode == SRC_DIRECT) return launch_wgrad_tc<15, SRC_DIRECT>(a, dz, dw, st);
-    if (ksize == 15 && mode == SRC_DECIM) return launch_wgrad_tc<15, SRC_DECIM>(a, dz, dw, st);
-    if (ksize == 5 && mode == SRC_UPCAT) return launch_wgrad_tc<5, SRC_UPCAT>(a, dz, dw, st);
+    if (ksize == 15 && mode == SRC_DIRECT) return launch_wgrad_tc<15, SRC_DIRECT>(a, dz, dw, st, slices);
+    if (ksize == 15 && mode == SRC_DECIM) return launch_wgrad_tc<15, SRC_DECIM>(a, dz, dw, st, slices);
+    if (ksize == 5 && mode == SRC_UPCAT) return launch_wgrad_tc<5, SRC_UPCAT>(a, dz, dw, st, slices);
     return -1;
 }
 

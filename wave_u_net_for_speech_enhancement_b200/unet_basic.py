@@ -136,7 +136,8 @@ class _NativeTrainStep(torch.autograd.Function):
     bn.bias) in forward order, then out.weight, out.bias.
 
     ``flags``: 0 = BatchNorm with batch statistics, running buffers updated (.train()); ``_lib.TRAIN_FROZEN_BN`` = BatchNorm
-    normalising by the running statistics, which stay untouched (.eval()). The backward fills the gradient of ``x`` when it
+    normalising by the running statistics, which stay untouched (.eval()); either may add ``_lib.TRAIN_DETERMINISTIC`` (weight
+    and head gradients summed in a fixed order, with a larger workspace). The backward fills the gradient of ``x`` when it
     requires grad and those of the parameters when any of them does; with no parameter requiring grad it computes ``dx``
     only (no weight-gradient pass, no reduction, no all-reduce)."""
 
@@ -153,7 +154,7 @@ class _NativeTrainStep(torch.autograd.Function):
         with torch.cuda.device(x.device):
             c = model._context(x.device)
             prec = _lib.PRECISIONS[model.train_precision]
-            nbytes = lib.wunet_train_workspace_bytes_prec(c, B, T, prec)
+            nbytes = lib.wunet_train_workspace_bytes_ex(c, B, T, prec, flags)
             if nbytes == 0:
                 _lib.check(-1)
             ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
@@ -254,6 +255,16 @@ class Model(nn.Module):
                    other eval forward takes the inference kernels (``precision``) and returns a detached tensor. "always" is
                    not the default because a caller that runs inference without ``torch.no_grad()`` (enhancement.py:66) would
                    then pay for the training kernels and their workspace on every call. Not part of the state_dict.
+
+    Deterministic mode (no constructor argument): a native training-kernel forward (``.train()``, or an eval forward that
+    records a graph) made while ``torch.backends.cudnn.deterministic`` or ``torch.are_deterministic_algorithms_enabled()``
+    is on sums the weight and head gradients in an order fixed by the shapes instead of with float atomics, and its
+    backward follows. The step is then bitwise repeatable (``y``, running buffers, every gradient, ``x.grad``) for the same
+    state, input, ``train_precision`` and GPU model. This is how the reference's ``"cudnn_deterministic": true``
+    (config/train/train.json, trainer/base_trainer.py:140-143) reaches the native step. It costs a scratch region in the
+    training workspace (about 70 MB in fp32, 22 MB in bf16 at the reference's batch of 120 x 16384). Note that
+    ``torch.use_deterministic_algorithms(True)`` also makes torch fill every ``torch.empty`` tensor, including the training
+    workspace, on every step (``torch.utils.deterministic.fill_uninitialized_memory``); that setting is left to the caller.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
@@ -414,7 +425,10 @@ class Model(nn.Module):
         for t in params:
             if t.device != x.device or t.dtype != torch.float32 or not t.is_contiguous():
                 raise RuntimeError("libwunet_b200 needs contiguous float32 parameters on the input's device")
-        y = _NativeTrainStep.apply(self, _lib.TRAIN_FROZEN_BN if frozen_bn else 0, self._aligned(x), *params)
+        flags = _lib.TRAIN_FROZEN_BN if frozen_bn else 0
+        if torch.backends.cudnn.deterministic or torch.are_deterministic_algorithms_enabled():
+            flags |= _lib.TRAIN_DETERMINISTIC
+        y = _NativeTrainStep.apply(self, flags, self._aligned(x), *params)
         if frozen_bn:
             return y                                         # running statistics untouched: the folded copies stay valid
         for blk in blocks:                                   # torch.nn.BatchNorm1d bookkeeping (momentum is not None: unused)
