@@ -38,6 +38,8 @@ extern "C" {
 #define WUNET_PREC_BF16 1   /* bf16 operands/activations, fp32 accumulate on wgmma tensor cores (config 3) */
 #define WUNET_PREC_FP32_TC 2 /* fp32-grade on the tensor cores: activations and weights split into bf16 high + low parts, three wgmma
                                MMAs per product (hi*hi + lo*hi + hi*lo, fp32 accumulate): <= 1e-4 vs the reference like WUNET_PREC_FP32 */
+#define WUNET_PREC_TF32 3   /* training step only: tf32 operands (round to nearest), fp32 accumulate on wgmma tensor cores; the
+                               inference entry points reject it (WUNET_EINVAL) */
 
 typedef struct wunet_ctx wunet_ctx;
 
@@ -199,6 +201,10 @@ int wunet_train_backward_part(wunet_ctx *ctx, const float *x, const float *y, co
  *                    accumulated in fp32 on the wgmma tensor cores; z, BatchNorm, the head, the decimate / upsample / concat
  *                    adjoints and all gradients stay fp32 (torch.autocast(bfloat16) semantics for Conv1d, except that z is fp32).
  *                    The first block (Cin = 1) stays fp32. Parameters and gradients are fp32 in the reference layouts.
+ *   WUNET_PREC_TF32  the same mixed-precision contract with tf32 operands: each is rounded to 11 significant bits (round to
+ *                    nearest, ties away from zero: cvt.rna.tf32.f32) and the products are accumulated in fp32 on wgmma
+ *                    (m64nNk8.f32.tf32.tf32). This is the arithmetic of cuDNN's Conv1d with torch.backends.cudnn.allow_tf32
+ *                    (PyTorch's default), i.e. of the reference's own training step on an H100. The first block stays fp32.
  *   WUNET_PREC_FP32_TC -> WUNET_EINVAL (not a training precision).
  * The backward must use the precision and workspace of its forward. Same call sites as above (trainer/trainer.py:35-37). */
 size_t wunet_train_workspace_bytes_prec(const wunet_ctx *ctx, int B, int T, int precision);
@@ -250,7 +256,7 @@ int wunet_train_backward_ex(wunet_ctx *ctx, const float *x, const float *y, cons
                             float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                             void *stream, float *dx, int part, int precision, int flags);
 /* Test hook, synchronous, on caller device buffers (fp32): one convolution-shaped pass of the training step at `precision`
- * (WUNET_PREC_FP32 or WUNET_PREC_BF16), the kernels the step itself uses. mode: 0 = direct, 1 = decimated (src0 is
+ * (WUNET_PREC_FP32, WUNET_PREC_BF16 or WUNET_PREC_TF32), the kernels the step itself uses. mode: 0 = direct, 1 = decimated (src0 is
  * [B][cin0][2L], every other sample read), 2 = upsample + concat (src0 = [B][cin0][L/2] interpolated 2x linearly,
  * align_corners=True, then src1 = [B][cin1][L]); ksize 15 with modes 0/1, 5 with mode 2 (pass 1 also takes 5 with mode 0).
  * w = [cout][cin0 + cin1][ksize] (Conv1d, no bias).
@@ -262,7 +268,7 @@ int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, 
                            const float *src0, const float *src1, const float *w, const float *dz, float *out);
 
 /* Introspection for tests, host-only (needs no GPU, no context): the training step of an n_layers / channels_interval model at
- * batch B, frame length T and training `precision` (WUNET_PREC_FP32 or WUNET_PREC_BF16), block `block` (0 .. 2*n_layers, forward
+ * batch B, frame length T and training `precision` (WUNET_PREC_FP32, _BF16 or _TF32), block `block` (0 .. 2*n_layers, forward
  * order). Writes 22 long longs (capacity >= 22):
  *  [0] z  [1] act  [2] ga  [3] mean  [4] invstd  [5] s1  [6] s2: byte offsets in the training workspace of the block's pre-BatchNorm
  *      output z [B][Cout][L], its activation [B][Cout][L], the activation gradient [B][Cout][L] (which holds dz after the
@@ -270,7 +276,7 @@ int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, 
  *      backward's mean(dy) and mean(dy * zhat) (written when that reduction runs)
  *  [7] Cin  [8] Cin0  [9] Cin1 (the skip channels of a decoder)  [10] Cout  [11] L  [12] ksize  [13] input mode (0 = the raw input,
  *      1 = the previous activation decimated, 2 = interpolated previous activation + skip)
- *  [14] weight-gradient kernel (0 = fp32 tiled, 1 = bf16 wgmma; block 0 is always 0)  [15] [16] [17] its gridDim x, y, z
+ *  [14] weight-gradient kernel (0 = fp32 tiled, 1 = bf16 wgmma, 2 = tf32 wgmma; block 0 is always 0)  [15] [16] [17] its gridDim x, y, z
  *  [18] (frame, position tile) work items shared by the gridDim.z slices  [19] positions per item  [20] largest number of items
  *      one CTA reduces  [21] wunet_train_workspace_bytes_prec for this B, T and precision.
  * No reference counterpart. */

@@ -1,10 +1,16 @@
-"""Training-step time of the reference architecture (n_layers 12, channels_interval 24, T = 16384) in five legs:
+"""Training-step time of the reference architecture (n_layers 12, channels_interval 24, T = 16384) in eight legs:
 
     native fp32   Model(train_backend="native", train_precision="fp32")   fp32 FFMA convolutions (wunet_train.cu)
     native bf16   Model(train_backend="native", train_precision="bf16")   bf16 wgmma convolutions (wunet_train_tc.cu)
-    *_det         the same two under torch.backends.cudnn.deterministic = True: deterministic mode (ordered weight- and
+    native tf32   Model(train_backend="native", train_precision="tf32")   tf32 wgmma convolutions (wunet_train_tf32.cu)
+    *_det         the same three under torch.backends.cudnn.deterministic = True: deterministic mode (ordered weight- and
                   head-gradient sums instead of float atomics)
     autocast      Model(train_backend="torch") under torch.autocast("cuda", torch.bfloat16): PyTorch eager + cuDNN
+    eager_tf32    Model(train_backend="torch") in fp32 with torch.backends.cudnn.allow_tf32 = True: PyTorch eager + cuDNN's
+                  TF32 convolutions, the reference's own arithmetic on an H100
+
+Each leg sets torch.backends.cudnn.allow_tf32 explicitly (CUDNN_TF32; True everywhere, PyTorch's default, which the legs
+before eager_tf32 were measured under) and restores it afterwards.
 
 Each step is what trainer/trainer.py:34-38 does: forward, MSE loss, backward, Adam (lr 1e-3; train.py:31-35). Per batch size
 every leg runs `--warmup` untimed steps and `--steps` timed ones, and the legs alternate over `--reps` repetitions. CUDA events
@@ -33,8 +39,13 @@ LEGS = {
     "native_fp32_det": dict(train_backend="native", train_precision="fp32"),
     "native_bf16": dict(train_backend="native", train_precision="bf16"),
     "native_bf16_det": dict(train_backend="native", train_precision="bf16"),
+    "native_tf32": dict(train_backend="native", train_precision="tf32"),
+    "native_tf32_det": dict(train_backend="native", train_precision="tf32"),
     "autocast_bf16": dict(train_backend="torch"),
+    "eager_tf32": dict(train_backend="torch"),
 }
+# torch.backends.cudnn.allow_tf32 per leg (only the eager legs run cuDNN convolutions; autocast's are bf16 anyway)
+CUDNN_TF32 = {leg: True for leg in LEGS}
 
 
 def gpu_info():
@@ -64,8 +75,9 @@ def run_steps(leg, state, n, timed):
     crit = torch.nn.MSELoss()
     ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(n)]
     losses = []
-    saved = torch.backends.cudnn.deterministic
+    saved = torch.backends.cudnn.deterministic, torch.backends.cudnn.allow_tf32
     torch.backends.cudnn.deterministic = leg.endswith("_det")
+    torch.backends.cudnn.allow_tf32 = CUDNN_TF32[leg]
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for i in range(n):
@@ -83,7 +95,7 @@ def run_steps(leg, state, n, timed):
         losses.append(loss.detach())
     torch.cuda.synchronize()
     wall = time.perf_counter() - t0
-    torch.backends.cudnn.deterministic = saved
+    torch.backends.cudnn.deterministic, torch.backends.cudnn.allow_tf32 = saved
     if not timed:
         return None
     ph = np.array([[e[0].elapsed_time(e[1]), e[1].elapsed_time(e[2]), e[2].elapsed_time(e[3])] for e in ev])
@@ -109,7 +121,8 @@ def main():
     os.makedirs(a.out, exist_ok=True)
     legs = a.legs.split(",")
     result = {"gpu_before": gpu_info(), "T": a.T, "warmup": a.warmup, "steps": a.steps, "reps": a.reps,
-              "torch": torch.__version__, "cudnn": torch.backends.cudnn.version(), "batches": {}}
+              "torch": torch.__version__, "cudnn": torch.backends.cudnn.version(),
+              "cudnn_allow_tf32": {leg: CUDNN_TF32[leg] for leg in legs}, "batches": {}}
     for B in [int(b) for b in a.batches.split(",")]:
         states = {leg: make_leg(leg, B, a.T) for leg in legs}
         for leg in legs:

@@ -10,7 +10,9 @@ SO_PATH = os.environ.get("WUNET_LIB_PATH") or os.path.join(_HERE, "libwunet_b200
 PREC_FP32 = 0
 PREC_BF16 = 1
 PREC_FP32_TC = 2
-PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC}
+PREC_TF32 = 3
+PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC}      # inference (Model(precision=...))
+TRAIN_PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32}      # training step (Model(train_precision=...))
 
 TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mode BatchNorm
 TRAIN_NO_PARAM_GRADS = 2   # backward: input gradient only
@@ -120,5 +122,6 @@ def debug_train_layout(n_layers: int, channels_interval: int, B: int, T: int, bl
     (host-only query: works without a GPU)."""
     n = len(TRAIN_LAYOUT_FIELDS)
     buf = (ctypes.c_longlong * n)()
-    check(load().wunet_debug_train_layout(n_layers, channels_interval, B, T, PRECISIONS[precision], block, buf, n))
+    code = TRAIN_PRECISIONS[precision] if precision in TRAIN_PRECISIONS else PRECISIONS[precision]   # fp32_tc: refused by the library
+    check(load().wunet_debug_train_layout(n_layers, channels_interval, B, T, code, block, buf, n))
     return dict(zip(TRAIN_LAYOUT_FIELDS, [int(v) for v in buf]))

@@ -292,7 +292,8 @@ size_t wunet_workspace_bytes(const wunet_ctx *c, int B, int T, int precision)
     }
     if (precision == WUNET_PREC_BF16) return tc_workspace_bytes(c->n, c->ci, B, T, 0);
     if (precision == WUNET_PREC_FP32_TC) return tc_workspace_bytes(c->n, c->ci, B, T, 1);
-    fail(WUNET_EINVAL, "unknown precision %d", precision);
+    if (precision == WUNET_PREC_TF32) fail(WUNET_EINVAL, "WUNET_PREC_TF32 is a training precision only (the forward has no tf32 path)");
+    else fail(WUNET_EINVAL, "unknown precision %d", precision);
     return 0;
 }
 
@@ -459,8 +460,10 @@ static int train_prec(int precision)
 {
     if (precision == WUNET_PREC_FP32) return TRAIN_FP32;
     if (precision == WUNET_PREC_BF16) return TRAIN_BF16;
+    if (precision == WUNET_PREC_TF32) return TRAIN_TF32;
     if (precision == WUNET_PREC_FP32_TC)
-        fail(WUNET_EINVAL, "training precision WUNET_PREC_FP32_TC is not supported: use WUNET_PREC_FP32 or WUNET_PREC_BF16");
+        fail(WUNET_EINVAL, "training precision WUNET_PREC_FP32_TC is not supported: use WUNET_PREC_FP32, WUNET_PREC_BF16 or "
+                           "WUNET_PREC_TF32");
     else
         fail(WUNET_EINVAL, "unknown training precision %d", precision);
     return -1;

@@ -90,4 +90,14 @@ WgradGrid wgrad_grid_bf16(int B, int L, int Cin, int Cout, int ksize);  // train
 size_t train_tc_packed_elems(int cout, int cin, int k);
 int train_tc_pack(const float *w, __nv_bfloat16 *wf, __nv_bfloat16 *wb, int Cout, int Cin, int K, cudaStream_t st);
 
+// ---- tf32 tensor-core training convolutions, implemented in wunet_train_tf32.cu ------------------------------
+// The same three operators as the bf16 launchers above, with tf32 operands (round to nearest, ties away: cvt.rna.tf32.f32);
+// a.wp points at the tf32 packing written by train_tf32_pack.
+int launch_conv_tf32(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
+int launch_wgrad_tf32(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices = false);
+WgradGrid wgrad_grid_tf32(int B, int L, int Cin, int Cout, int ksize);  // train_wgrad_tf32_kernel
+// fp32 elements of one tf32 packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout))
+size_t train_tf32_packed_elems(int cout, int cin, int k);
+int train_tf32_pack(const float *w, float *wf, float *wb, int Cout, int Cin, int K, cudaStream_t st);
+
 }  // namespace wunet

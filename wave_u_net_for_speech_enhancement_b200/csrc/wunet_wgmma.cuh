@@ -1,5 +1,6 @@
 // wunet_wgmma.cuh — sm_90a device helpers shared by the tensor-core kernels (wunet_tc.cu: inference forward;
-// wunet_train_tc.cu: bf16 training convolutions). Raw PTX; forms taken from the PTX ISA as shipped in CUDA 12.9.
+// wunet_train_tc.cu: bf16 training convolutions; wunet_train_tf32.cu: tf32 training convolutions). Raw PTX; forms taken
+// from the PTX ISA as shipped in CUDA 12.9.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -181,6 +182,78 @@ template <int N, int TA = 0, int TB = 0>
 __device__ __forceinline__ void wgmma_m64nNk16(float (&d)[N / 2], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
 {
     WgmmaBf16<N, TA, TB>::mma(d, a_lo, b_lo, hi);
+}
+
+// D[64 x N] += A[64 x 8] * B[N x 8]^T, tf32 operands (fp32 words; the MMA reads the top 19 bits), fp32 accumulators,
+// N = 16 .. 64. Both operands K-major: the PTX has no transpose immediates for 32-bit operand types. A 128-byte swizzled row
+// holds 32 fp32 K elements, so one K8 step is 32 bytes, the same descriptor advance as a bf16 K16 step. Same f32 fragment as
+// wgmma_m64nNk16.
+template <int N> struct WgmmaTf32;
+template <> struct WgmmaTf32<16> {
+    static __device__ __forceinline__ void mma(float (&d)[8], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%8, %10};\n\tmov.b64 db, {%9, %10};\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {"
+            "%0, %1, %2, %3, %4, %5, %6, %7"
+            "}, da, db, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "r"(a_lo), "r"(b_lo), "r"(hi)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32<32> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%16, %18};\n\tmov.b64 db, {%17, %18};\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+            "}, da, db, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a_lo), "r"(b_lo), "r"(hi)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32<48> {
+    static __device__ __forceinline__ void mma(float (&d)[24], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%24, %26};\n\tmov.b64 db, {%25, %26};\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23"
+            "}, da, db, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "r"(a_lo), "r"(b_lo), "r"(hi)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, 1, 0;\n\tmov.b64 da, {%32, %34};\n\tmov.b64 db, {%33, %34};\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+            "}, da, db, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a_lo), "r"(b_lo), "r"(hi)
+            : "memory");
+    }
+};
+
+template <int N>
+__device__ __forceinline__ void wgmma_m64nNk8_tf32(float (&d)[N / 2], uint32_t a_lo, uint32_t b_lo, uint32_t hi)
+{
+    WgmmaTf32<N>::mma(d, a_lo, b_lo, hi);
 }
 
 }  // namespace

@@ -153,7 +153,7 @@ class _NativeTrainStep(torch.autograd.Function):
         B, _, T = x.shape
         with torch.cuda.device(x.device):
             c = model._context(x.device)
-            prec = _lib.PRECISIONS[model.train_precision]
+            prec = _lib.TRAIN_PRECISIONS[model.train_precision]
             nbytes = lib.wunet_train_workspace_bytes_ex(c, B, T, prec, flags)
             if nbytes == 0:
                 _lib.check(-1)
@@ -242,8 +242,11 @@ class Model(nn.Module):
                    gradient, weight gradient). "fp32" (default): fp32 FFMA. "bf16": mixed precision — their operands (block
                    input, weights, dz) are rounded to bf16 and the products accumulated in fp32 on the tensor cores; z,
                    BatchNorm, the head and all gradients stay fp32, parameters stay fp32 (the caller's optimizer is unchanged).
-                   ``torch.autocast(bfloat16)`` semantics for Conv1d, except that z is kept in fp32. Only with
-                   train_backend="native". Not part of the state_dict.
+                   ``torch.autocast(bfloat16)`` semantics for Conv1d, except that z is kept in fp32. "tf32": the same with
+                   the operands rounded to tf32 (11 significant bits, round to nearest) instead, which is what cuDNN does
+                   for Conv1d on an H100 under PyTorch's default ``torch.backends.cudnn.allow_tf32 = True``, i.e. the
+                   reference's own training arithmetic there (that flag does not select it: the default stays "fp32").
+                   "bf16" and "tf32" only with train_backend="native". Not part of the state_dict.
     eval_autograd  when an eval-mode forward records an autograd graph (grad mode on, train_backend "native" or "torch").
                    "input" (default): when the input requires grad — ``x.grad`` of an upstream model or front end, input
                    gradients of an adversarial perturbation. "always": also when some parameter requires grad, for
@@ -279,8 +282,8 @@ class Model(nn.Module):
         self.channels_interval = channels_interval
         if data_parallel not in ("auto", "off"):
             raise ValueError("data_parallel must be 'auto' or 'off'")
-        if train_precision not in ("fp32", "bf16"):
-            raise ValueError(f"train_precision must be 'fp32' or 'bf16', got {train_precision!r}")
+        if train_precision not in _lib.TRAIN_PRECISIONS:
+            raise ValueError(f"train_precision must be one of {sorted(_lib.TRAIN_PRECISIONS)}, got {train_precision!r}")
         if train_precision != "fp32" and train_backend != "native":
             raise ValueError(f"train_precision={train_precision!r} needs train_backend='native' (got {train_backend!r})")
         if eval_autograd not in ("input", "always", "off"):
@@ -406,7 +409,7 @@ class Model(nn.Module):
         training) and of ``x`` when it requires grad; the caller's optimizer is used unchanged (trainer/trainer.py:34-38).
         BatchNorm uses batch statistics and updates its running buffers (.train()) or, with ``frozen_bn``, normalises by the
         running statistics and leaves them and ``num_batches_tracked`` untouched (.eval()). fp32 or, with
-        ``train_precision="bf16"``, bf16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
+        ``train_precision="bf16"`` / ``"tf32"``, bf16 / tf32 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
         B, _, T = x.shape
         if not frozen_bn and B * (T >> self.n_layers) == 1:
