@@ -1,5 +1,5 @@
-"""Teacher-forced check of every kernel of the native training step (csrc/wunet_train.cu, csrc/wunet_train_tc.cu), block by
-block, against float64.
+"""Teacher-forced check of every kernel of the native training step (csrc/wunet_train.cu, csrc/wunet_train_tc.cu,
+csrc/wunet_train_tf32.cu), block by block, against float64.
 
 The step runs through wunet_train_forward_ex / wunet_train_backward_ex on a workspace this test allocates; every block's
 tensors are read as views given by the host-only layout query (wunet_debug_train_layout). For each block, what its kernels
@@ -16,10 +16,15 @@ that fits its own arithmetic:
   sums whose value can be cancellation noise.
 - dz: the bar of the routed activation gradient propagated through the BatchNorm backward, plus its own fp32 roundings.
 - the head (1x1 conv + tanh) and its gradients (warp sums + atomicAdd over B * T samples): see HEAD_REL.
-In bf16 mode the reference convolves the bf16-rounded operands the kernels multiply. An interpolated operand (decoder input)
-is computed in fp32 first; the kernel's value may differ from the exactly rounded one by its own rounding (|err| <= 2^-23
-of |lam0 a| + |lam1 b|), and where that interval straddles a bf16 rounding boundary the operand may round to the other bf16
-neighbour: the bar adds that interval, weighted like the products it enters.
+In bf16 and tf32 mode the reference convolves the operands the kernels multiply, rounded as they round them (bf16: nearest
+even; tf32: cvt.rna, nearest with ties away from zero), block by block as the layout query reports the block's kernels. An
+interpolated operand (decoder input) is computed in fp32 first; the kernel's value may differ from the exactly rounded one by
+its own rounding (|err| <= 2^-23 of |lam0 a| + |lam1 b|), and where that interval straddles a rounding boundary the operand
+may round to the other neighbour: the bar adds that interval, weighted like the products it enters.
+
+In the runs of BN_REDUCTION the BatchNorm backward reductions of the middle block are also held to one fp32 ulp
+(check_bn_reduction): its activation gradient is final after part 0 of the split backward, so a copy taken between the parts
+is the exact input of train_bn_bwd_stats / train_bn_bwd_apply, whose fp32 arithmetic is replayed from it.
 
 The worst error/bar ratio of every quantity is printed per block, so the margins are on record (DESIGN §3)."""
 import ctypes
@@ -39,19 +44,30 @@ pytestmark = [pytest.mark.gpu]
 # backward computes parameter gradients (False: WUNET_TRAIN_NO_PARAM_GRADS, dx only)
 CASES = {
     # the reference's own config/train (batch_size 120, sample_length 16384): fp32 weight gradient 4-52 tiles per CTA, bf16
-    # 14-233 items per CTA, BatchNorm reductions over ~2M samples per channel
-    "production": dict(n=12, ci=24, B=120, T=16384, precisions=("fp32", "bf16"), modes=("batch",), param_grads=(True,)),
-    # L = 5 * 2^k: partial 128-position tiles (L = 320, 160), partial 64-position chunks (L = 160, 80), 5 -> 10 upsampling
-    "odd_lengths": dict(n=12, ci=24, B=3, T=20480, precisions=("fp32", "bf16"), modes=("batch", "frozen"), param_grads=(True,)),
-    # channel counts that are not multiples of 8, 16 or 64 (partial co / ci tiles of both weight-gradient kernels)
-    "channel_plan": dict(n=6, ci=20, B=5, T=2048, precisions=("fp32", "bf16"), modes=("batch",), param_grads=(True,)),
+    # and tf32 14-233 items per CTA, BatchNorm reductions over ~2M samples per channel
+    "production": dict(n=12, ci=24, B=120, T=16384, precisions=("fp32", "bf16", "tf32"), modes=("batch",), param_grads=(True,)),
+    # L = 5 * 2^k: partial 128-position tiles (L = 320, 160), partial 64-position chunks (L = 160, 80), frames shorter than 64
+    # samples, 5 -> 10 upsampling
+    "odd_lengths": dict(n=12, ci=24, B=3, T=20480, precisions=("fp32", "bf16", "tf32"), modes=("batch", "frozen"),
+                        param_grads=(True,)),
+    # channel counts that are not multiples of 8, 16, 32 or 64 (partial co / ci tiles of the weight-gradient kernels, padded
+    # 32-channel K chunks of the tf32 forward)
+    "channel_plan": dict(n=6, ci=20, B=5, T=2048, precisions=("fp32", "bf16", "tf32"), modes=("batch",), param_grads=(True,)),
+    # a middle block with 32 x 1024 = 32768 values per channel (480 at the production shape) for the BatchNorm reductions, and
+    # Cout = 8 blocks on the tensor-core kernels, whose tiles are mostly padding
+    "long_middle": dict(n=4, ci=8, B=32, T=16384, precisions=("fp32", "bf16", "tf32"), modes=("batch",), param_grads=(True,)),
     # B = 1: BatchNorm over L only, two values per channel at the middle block
     "one_frame": dict(n=12, ci=24, B=1, T=8192, precisions=("fp32",), modes=("batch",), param_grads=(True,)),
     # L = 1 with B = 1 at the middle block, which eval-mode BatchNorm allows; with and without parameter gradients
     "one_value": dict(n=12, ci=24, B=1, T=4096, precisions=("fp32",), modes=("frozen",), param_grads=(True, False)),
 }
 # (case, precision) whose backward also runs as part 0 followed by part 1 (the data-parallel split) on a copy of the workspace
-SPLIT = {("production", "fp32"), ("odd_lengths", "bf16")}
+SPLIT = {("production", "fp32"), ("odd_lengths", "bf16"), ("production", "tf32")}
+# runs (case, precision, mode, parameter gradients) whose middle block's BatchNorm backward is also replayed to one fp32 ulp
+# from a copy of its activation gradient taken between part 0 and part 1; they run the split backward even if not in SPLIT
+BN_REDUCTION = ([("production", p, "batch", True) for p in ("fp32", "bf16", "tf32")] +
+                [("long_middle", p, "batch", True) for p in ("fp32", "bf16", "tf32")] +
+                [("odd_lengths", p, "frozen", True) for p in ("fp32", "bf16", "tf32")])
 
 U32 = 2.0 ** -24                    # unit roundoff of fp32
 U = 4 * U32                         # what the bars count per fp32 rounding of an elementwise formula: 4x its unit roundoff
@@ -61,9 +77,11 @@ SLOPE = float(np.float32(0.1))      # kLreluSlope
 MOMENTUM = 0.1
 CONV_REL = 1e-5     # fp32 accumulation of <= 4320 products: worst case n u ~ 2.6e-4 of sum |products|
 # weight gradients, a sum over B * L positions: fp32 FFMA chains of up to 52 x 128 positions per thread, then atomicAdd over
-# the gridDim.z slices (measured <= 1e-6 of sum |products|); bf16: wgmma's fp32 accumulation over up to 233 x 64 positions
-# per CTA (measured <= 9.4e-5). Staging dz of the wrong tile moves outputs by 0.2-0.6 of sum |products|.
-WGRAD_REL = {"fp32": 1e-5, "bf16": 1e-3}
+# the gridDim.z slices (measured <= 1e-6 of sum |products|); bf16 and tf32: wgmma's fp32 accumulation over up to 233 x 64
+# positions per CTA (measured <= 9.4e-5 bf16, <= 3.4e-5 tf32 at the production shape, H100 80GB HBM3 at 700 W). Staging dz
+# of the wrong tile moves outputs by 0.2-0.6 of sum |products|; tf32 operands truncated instead of rounded to nearest, by
+# ~7e-4 at the production shape.
+WGRAD_REL = {"fp32": 1e-5, "bf16": 1e-3, "tf32": 3e-4}
 HEAD_REL = 1e-4     # 1x1 head gradients: fp32 products, warp sums, then one atomicAdd per warp over B * T / 32 warps
 DOUBLE_REL = 1e-12  # double reductions of fp32 values: summation-order noise relative to the sum of magnitudes
 
@@ -91,6 +109,18 @@ def ulp32(v):
 def bf16r(v):
     """Round to bf16 (nearest even) the fp32 value the kernels hold, back in float64."""
     return v.float().bfloat16().double()
+
+
+def tf32r(v):
+    """cvt.rna.tf32.f32 of the fp32 value the kernels hold (round to nearest, ties away from zero: add half of the 13 dropped
+    bits to the magnitude's bit pattern, then clear them), back in float64. On the tensor's device: the block tensors of the
+    production case hold tens of millions of elements."""
+    u = v.float().contiguous().view(torch.int32)
+    return ((u + 0x1000) & -8192).view(torch.float32).double()
+
+
+# operand rounding of a block's convolution kernels by the layout query's wgrad_tc: CUDA cores (none), bf16 or tf32 tensor cores
+ROUND = {0: None, 1: bf16r, 2: tf32r}
 
 
 def fma32(a, b, c):
@@ -199,7 +229,7 @@ class Step:
         self.lib = _lib.load()
         self.ctx = ctypes.c_void_p()
         _lib.check(self.lib.wunet_create(n, ci, 0, ctypes.byref(self.ctx)))
-        nbytes = self.lib.wunet_train_workspace_bytes_prec(self.ctx, B, T, _lib.PRECISIONS[prec])
+        nbytes = self.lib.wunet_train_workspace_bytes_prec(self.ctx, B, T, _lib.TRAIN_PRECISIONS[prec])
         assert nbytes == self.lay[0]["workspace_bytes"]
         self.ws = torch.full((nbytes // 4,), float("nan"), dtype=torch.float32, device=dev)   # unwritten reads show as NaN
         self.y = torch.full_like(self.x, float("nan"))
@@ -217,7 +247,7 @@ class Step:
         return self.lib.wunet_train_forward_ex(self.ctx, self.x.data_ptr(), self.y.data_ptr(), self.B, self.T, P(self.w),
                                                P(self.b), P(self.gamma), P(self.beta), P(self.rm), P(self.rv),
                                                self.wo.data_ptr(), self.bo.data_ptr(), MOMENTUM, self.ws.data_ptr(),
-                                               self.ws.numel() * 4, None, _lib.PRECISIONS[self.prec], self.flags)
+                                               self.ws.numel() * 4, None, _lib.TRAIN_PRECISIONS[self.prec], self.flags)
 
     def new_grads(self):
         if not self.pgrads:
@@ -234,7 +264,7 @@ class Step:
             self.ctx, self.x.data_ptr(), self.y.data_ptr(), self.dy.data_ptr(), self.B, self.T, P(self.w), P(self.gamma),
             P(self.beta), self.wo.data_ptr(), P(g.get("w")), P(g.get("b")), P(g.get("gamma")), P(g.get("beta")),
             g["wo"].data_ptr() if G else None, g["bo"].data_ptr() if G else None, ws.data_ptr(), ws.numel() * 4, None,
-            None if dx is None else dx.data_ptr(), part, _lib.PRECISIONS[self.prec], flags))
+            None if dx is None else dx.data_ptr(), part, _lib.TRAIN_PRECISIONS[self.prec], flags))
 
     def view(self, ws, i, field):
         d = self.lay[i]
@@ -242,8 +272,13 @@ class Step:
         o = d[field] // 4
         return ws[o:o + int(np.prod(shape))].view(shape)
 
-    def tc(self, i):
-        return self.lay[i]["wgrad_tc"] == 1
+    def rnd(self, i):
+        """The operand rounding of block i's convolution kernels, or None (fp32 operands)."""
+        return ROUND[self.lay[i]["wgrad_tc"]]
+
+    def rounded(self, i, v):
+        r = self.rnd(i)
+        return v if r is None else r(v)
 
     def block_input(self, i):
         """-> (float64 block input as the block's kernels see it, rounding allowance of each operand or None, upsample data)."""
@@ -258,15 +293,15 @@ class Step:
             skip = self.view(self.ws, 2 * self.n - i, "act").double()
             xin = torch.cat([v, skip], 1)
             xu = torch.cat([delta, torch.zeros_like(skip)], 1)
-        if self.tc(i):
+        r = self.rnd(i)
+        if r is not None:
             if xu is not None:
-                xu = bf16r(xin + xu) - bf16r(xin - xu)
-            xin = bf16r(xin)
+                xu = r(xin + xu) - r(xin - xu)
+            xin = r(xin)
         return xin, xu, up
 
     def weight(self, i):
-        w = self.w[i].double()
-        return bf16r(w) if self.tc(i) else w
+        return self.rounded(i, self.w[i].double())
 
 
 def check_forward(s, rep):
@@ -390,7 +425,7 @@ def check_backward(s, rep, wss, gsets, dxs):
             for G in gsets[1:]:
                 rep.equal(i, "g_conv_b (part split)", G["b"][i], gsets[0]["b"][i])
             xin, xu, _ = s.block_input(i)
-            dzr = bf16r(dzd) if s.tc(i) else dzd
+            dzr = s.rounded(i, dzd)
             want = torch.nn.grad.conv1d_weight(xin, s.w[i].shape, dzr, padding=pad)
             bar = WGRAD_REL[s.prec] * torch.nn.grad.conv1d_weight(xin.abs(), s.w[i].shape, dzr.abs(), padding=pad)
             if xu is not None:
@@ -409,7 +444,7 @@ def check_backward(s, rep, wss, gsets, dxs):
             continue
         # input gradient of the block, routed to the producers of its input (decimation / interpolation + concat adjoints)
         W = s.weight(i)
-        dzr = bf16r(dzd) if s.tc(i) else dzd
+        dzr = s.rounded(i, dzd)
         din = F.conv_transpose1d(dzr, W, padding=pad)
         e_din = CONV_REL * F.conv_transpose1d(dzr.abs(), W.abs(), padding=pad)
         del dzr, dzd
@@ -437,12 +472,43 @@ def check_backward(s, rep, wss, gsets, dxs):
     assert not pending
 
 
+def check_bn_reduction(s, rep, ws, G, ga):
+    """The BatchNorm backward of the middle block (n), replayed in the kernels' fp32 arithmetic from `ga`, a copy of its
+    activation gradient taken between part 0 and part 1 (the exact input of train_bn_bwd_stats and train_bn_bwd_apply; ws and
+    G are the workspace and gradients that run finished in). No error bar is inherited from the routed gradient:
+    - s1 = mean(dy), s2 = mean(dy zh) and the parameter gradients g_bn_bias = sum dy, g_bn_weight = sum dy zh are double sums of
+      fp32 terms (dy zh is exact in double), rounded once: 1 fp32 ulp + DOUBLE_REL of the sum of magnitudes. A float
+      accumulator instead of a double one, or a dropped term, shows as many ulps.
+    - dz = fp32(invstd gamma) * (dy - s1 - zh s2) from the native s1, s2 (zeros with frozen statistics): the kernel's formula,
+      with zh s2 contracted into an FMA (the compiled train_bn_bwd_apply_kernel's FFMA), replayed exactly; 2 ulps."""
+    i = s.n
+    cnt = s.B * s.lay[i]["L"]
+    z, mean, invstd = s.view(ws, i, "z"), s.view(ws, i, "mean"), s.view(ws, i, "invstd")
+    zh, yv = bn_replay(z, mean, invstd, s.gamma[i], s.beta[i])
+    dyv = torch.where(yv >= 0, ga, torch.tensor(SLOPE, dtype=torch.float32, device=s.dev) * ga)
+    del yv
+    d, zd = dyv.double(), zh.double()
+    for name, terms, gname, gkey in (("s1", d, "g_bn_bias", "beta"), ("s2", d * zd, "g_bn_weight", "gamma")):
+        t, mag = terms.sum((0, 2)), terms.abs().sum((0, 2))
+        rep.check(i, name + " (1 ulp)", s.view(ws, i, name), t / cnt, ulp32(t / cnt) + DOUBLE_REL * mag / cnt)
+        if G is not None:
+            rep.check(i, gname + " (1 ulp)", G[gkey][i], t, ulp32(t) + DOUBLE_REL * mag)
+        del terms
+    del d, zd
+    c = lambda t: t[None, :, None].expand_as(z)          # noqa: E731
+    zeros = torch.zeros_like(mean)
+    s1, s2 = (zeros, zeros) if s.frozen else (s.view(ws, i, "s1"), s.view(ws, i, "s2"))
+    want = (c(invstd) * c(s.gamma[i])) * fma32(-zh, c(s2), dyv - c(s1))
+    rep.check(i, "dz (replay)", s.view(ws, i, "ga"), want.double(), 2 * ulp32(want.double()))
+
+
 @pytest.mark.parametrize("run", RUNS, ids=[_run_id(r) for r in RUNS])
 def test_training_kernels_block_by_block(run):
     case, prec, mode, pgrads = run
     t0 = time.perf_counter()
     s = Step(case, prec, mode, pgrads)
-    split = (case, prec) in SPLIT
+    bnred = run in BN_REDUCTION
+    split = (case, prec) in SPLIT or bnred
     wss, gsets, dxs = [s.ws], [s.new_grads()], [torch.full_like(s.x, float("nan"))]
     if split:
         wss.append(s.ws.clone())                          # the backward turns ga into dz in place
@@ -451,6 +517,7 @@ def test_training_kernels_block_by_block(run):
     s.backward(wss[0], gsets[0], dxs[0], -1)
     if split:
         s.backward(wss[1], gsets[1], None, 0)
+        ga_mid = s.view(wss[1], s.n, "ga").clone() if bnred else None     # final after part 0: the middle block feeds dec0 only
         s.backward(wss[1], gsets[1], dxs[1], 1)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
@@ -458,6 +525,8 @@ def test_training_kernels_block_by_block(run):
     with torch.no_grad():
         check_forward(s, rep)
         check_backward(s, rep, wss, gsets, dxs)
+        if bnred:
+            check_bn_reduction(s, rep, wss[1], gsets[1], ga_mid)
     torch.cuda.synchronize()
     _lib.load().wunet_destroy(s.ctx)
     rep.print()

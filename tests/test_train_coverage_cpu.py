@@ -3,11 +3,14 @@ the training kernels can go wrong. This guard reads its case table through the h
 every block's workspace regions are sound, and together the cases reach
 
 - the fp32 weight gradient with >= 32 tiles per CTA (the tile loop) and with exactly one;
-- the bf16 weight gradient with >= 100 items per CTA and with exactly one;
-- a frame whose last 128-position (fp32) or 64-position (bf16) tile is partial;
+- the bf16 and the tf32 weight gradient each with >= 100 items per CTA and with exactly one;
+- a frame whose last 128-position (fp32) or 64-position (bf16, tf32) tile is partial;
 - frames of fewer than 4 samples (the zero padding of the fp32 weight gradient's 4-position inner step);
-- Cout not a multiple of 16 and Cin not a multiple of 64 (partial co / ci tiles);
-- B = 1, frozen BatchNorm, a backward without parameter gradients, and the part 0 / part 1 split.
+- Cout not a multiple of 16 and Cin not a multiple of 64 (partial co / ci tiles), and a tf32 block whose Cin is not a
+  multiple of 32 (a padded 32-channel K chunk of the tf32 forward);
+- B = 1, frozen BatchNorm, a backward without parameter gradients, and the part 0 / part 1 split;
+- the one-ulp replay of the middle block's BatchNorm backward reductions over >= 32768 values per channel, and with frozen
+  statistics.
 
 It fails as soon as a change of the case table or of the launch geometry drops one of them."""
 import ctypes
@@ -18,9 +21,11 @@ import test_train_blocks_gpu as blocks
 from wave_u_net_for_speech_enhancement_b200 import _lib
 
 REQUIRED = {"fp32_wgrad_ge_32_per_cta", "fp32_wgrad_1_per_cta", "bf16_wgrad_ge_100_per_cta", "bf16_wgrad_1_per_cta",
-            "partial_tile", "frame_lt_4", "cout_not_mult_16", "cin_not_mult_64", "batch_1", "frozen", "no_param_grads",
-            "part_split"}
+            "tf32_wgrad_ge_100_per_cta", "tf32_wgrad_1_per_cta", "tf32_cin_not_mult_32", "partial_tile", "frame_lt_4",
+            "cout_not_mult_16", "cin_not_mult_64", "batch_1", "frozen", "no_param_grads", "part_split",
+            "bn_reduction_ge_32768_per_channel", "bn_reduction_frozen"}
 FIELDS = ("z", "act", "ga", "mean", "invstd", "s1", "s2")
+KIND = {0: "fp32", 1: "bf16", 2: "tf32"}      # wgrad_tc: the weight-gradient kernel of a block
 
 
 def regions(d, B):
@@ -36,7 +41,7 @@ def layouts(case, prec):
 @pytest.mark.parametrize("case", sorted(blocks.CASES))
 def test_layout_regions_are_disjoint_aligned_and_inside_the_workspace(case):
     c = blocks.CASES[case]
-    for prec in ("fp32", "bf16"):
+    for prec in ("fp32", "bf16", "tf32"):
         lay = layouts(case, prec)
         total = lay[0]["workspace_bytes"]
         spans = []
@@ -47,30 +52,36 @@ def test_layout_regions_are_disjoint_aligned_and_inside_the_workspace(case):
                 spans.append((off, off + size))
         spans.sort()
         assert all(a[1] <= b[0] for a, b in zip(spans, spans[1:])), (case, prec)
-    fp32, bf16 = layouts(case, "fp32"), layouts(case, "bf16")
-    for a, b in zip(fp32, bf16):
-        assert {f: a[f] for f in FIELDS} == {f: b[f] for f in FIELDS}
-    assert fp32[0]["workspace_bytes"] <= bf16[0]["workspace_bytes"]
+    fp32 = layouts(case, "fp32")
+    for prec in ("bf16", "tf32"):
+        other = layouts(case, prec)
+        for a, b in zip(fp32, other):
+            assert {f: a[f] for f in FIELDS} == {f: b[f] for f in FIELDS}, (case, prec)
+        assert fp32[0]["workspace_bytes"] <= other[0]["workspace_bytes"], (case, prec)
 
 
 def test_layout_query_describes_the_channel_plan_and_the_weight_gradient_launch():
     n, ci, B, T = 12, 24, 120, 16384
-    for prec in ("fp32", "bf16"):
+    for prec in ("fp32", "bf16", "tf32"):
         for i in range(2 * n + 1):
             d = _lib.debug_train_layout(n, ci, B, T, i, prec)
             L = T >> i if i <= n else T >> (2 * n - i)
             assert (d["L"], d["ksize"], d["mode"]) == (L, 15 if i <= n else 5, 0 if i == 0 else 1 if i <= n else 2)
             assert d["Cin"] == d["Cin0"] + d["Cin1"] and (d["Cin1"] > 0) == (i > n)
-            assert d["wgrad_tc"] == (1 if prec == "bf16" and i > 0 else 0)
+            assert d["wgrad_tc"] == ({"fp32": 0, "bf16": 1, "tf32": 2}[prec] if i > 0 else 0)
             tiles = -(-L // d["positions"])
             assert d["items"] == B * tiles and d["items_per_cta"] == -(-d["items"] // d["grid_z"])
             if d["wgrad_tc"]:
                 assert d["positions"] == 64 and d["grid_x"] == -(-d["Cout"] // 64) * (d["ksize"] // 5)
+                if d["wgrad_tc"] == 2:
+                    assert d["grid_y"] == -(-d["Cin"] // 64)
             else:
                 assert d["positions"] == min(L, 128) and (d["grid_x"], d["grid_y"]) == (-(-d["Cout"] // 16), -(-d["Cin"] // 64))
     fp32 = [_lib.debug_train_layout(n, ci, B, T, i, "fp32")["items_per_cta"] for i in range(2 * n + 1)]
     bf16 = [_lib.debug_train_layout(n, ci, B, T, i, "bf16")["items_per_cta"] for i in range(1, 2 * n + 1)]
+    tf32 = [_lib.debug_train_layout(n, ci, B, T, i, "tf32")["items_per_cta"] for i in range(1, 2 * n + 1)]
     assert (min(fp32), max(fp32), min(bf16), max(bf16)) == (4, 52, 14, 233)
+    assert (min(tf32), max(tf32)) == (14, 233)                # dec11: 30720 items over 132 slices
     for bad in [(12, 24, 2, 4096, 25, "fp32"), (12, 24, 2, 4000, 0, "fp32"), (12, 24, 2, 4096, 0, "fp32_tc")]:
         with pytest.raises(_lib.WunetError):
             _lib.debug_train_layout(*bad)
@@ -81,12 +92,15 @@ def test_layout_query_describes_the_channel_plan_and_the_weight_gradient_launch(
 def features(case, prec, mode, pgrads):
     c = blocks.CASES[case]
     f = set()
-    for d in layouts(case, prec):
-        kind = "bf16" if d["wgrad_tc"] else "fp32"
+    lay = layouts(case, prec)
+    for d in lay:
+        kind = KIND[d["wgrad_tc"]]
         if d["items_per_cta"] == 1:
             f.add(f"{kind}_wgrad_1_per_cta")
-        if d["items_per_cta"] >= (100 if kind == "bf16" else 32):
-            f.add(f"{kind}_wgrad_ge_{100 if kind == 'bf16' else 32}_per_cta")
+        if d["items_per_cta"] >= (32 if kind == "fp32" else 100):
+            f.add(f"{kind}_wgrad_ge_{32 if kind == 'fp32' else 100}_per_cta")
+        if kind == "tf32" and d["Cin"] % 32 != 0:
+            f.add("tf32_cin_not_mult_32")
         if d["L"] % d["positions"] != 0:
             f.add("partial_tile")
         if d["L"] < 4:
@@ -103,7 +117,19 @@ def features(case, prec, mode, pgrads):
         f.add("no_param_grads")
     if (case, prec) in blocks.SPLIT:
         f.add("part_split")
+    if (case, prec, mode, pgrads) in blocks.BN_REDUCTION:
+        mid = lay[c["n"]]
+        if c["B"] * mid["L"] >= 32768:
+            f.add("bn_reduction_ge_32768_per_channel")
+        if mode == "frozen":
+            f.add("bn_reduction_frozen")
     return f
+
+
+def test_bn_reduction_runs_are_runs_with_parameter_gradients():
+    """The replay checks the BatchNorm parameter gradients, so every run it names must exist and compute them."""
+    for r in blocks.BN_REDUCTION:
+        assert r in blocks.RUNS and r[3], r
 
 
 def test_cases_reach_every_training_regime():

@@ -11,6 +11,7 @@ import torch.nn.functional as F
 
 import test_autograd_gpu as tag
 import test_train_bf16_gpu as tbf
+import test_train_blocks_gpu as tbl
 import test_train_deterministic_gpu as tdet
 from oracle import wunet_oracle as wo
 from wave_u_net_for_speech_enhancement_b200 import Model, _lib
@@ -42,6 +43,26 @@ def test_tf32_emulation_is_round_to_nearest_ties_away():
     half = np.float32(2.0 ** -11)               # half a tf32 ulp at 1
     got = tf32(np.array([1 + half, -(1 + half), 1 + half / 2, 1 + 1.5 * half], dtype=np.float32)).numpy()
     assert list(got) == [1 + 2 * half, -(1 + 2 * half), one, 1 + 2 * half]
+
+
+def test_gpu_rounding_matches_the_emulation():
+    """test_train_blocks_gpu.tf32r (the same rounding on int32 views of CUDA tensors, for the block check's tens of millions of
+    operands) against tf32() above, bit for bit: ties and their neighbours in both signs, subnormals, the top of a binade
+    (rounding up into the next one), the largest finite values (rounding up to infinity), zeros and random bit patterns."""
+    pats = [0x3F801000, 0x3F800FFF, 0x3F801001, 0x3F803000, 0x3F802FFF,          # ties at 1 (odd and even kept bit), neighbours
+            0x00000001, 0x00000FFF, 0x00001000, 0x00001FFF, 0x00003000, 0x007FF000, 0x007FFFFF,   # subnormals
+            0x3FFFEFFF, 0x3FFFF000, 0x3FFFFFFF, 0x407FF000,                       # the top of a binade
+            0x7F7FEFFF, 0x7F7FF000, 0x7F7FFFFF, 0x00000000, 0x00800000, 0x3DCCCCCD]
+    rng = np.random.default_rng(3)
+    exps = rng.integers(0, 255, 4096, dtype=np.uint32) << np.uint32(23)      # finite exponents, including subnormals
+    bits = np.concatenate([np.array(pats, dtype=np.uint32), exps | rng.integers(0, 1 << 23, 4096, dtype=np.uint32)])
+    bits = np.concatenate([bits, bits | np.uint32(0x80000000)])
+    vals = bits.view(np.float32)
+    want = tf32(vals).numpy().astype(np.float32).view(np.uint32)
+    got = tbl.tf32r(torch.from_numpy(vals).cuda()).float().cpu().numpy().view(np.uint32)
+    bad = np.flatnonzero(got != want)
+    assert bad.size == 0, [(hex(bits[i]), hex(got[i]), hex(want[i])) for i in bad[:10]]
+    assert want[0] == 0x3F802000 and want[1] == 0x3F800000 and want[18] == 0x7F800000     # ties away; top rounds to inf
 
 
 def run_pass(pss, mode, k, B, L, cin0, cin1, cout, src0, src1, w, dz):
