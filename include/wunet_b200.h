@@ -40,6 +40,13 @@ extern "C" {
                                MMAs per product (hi*hi + lo*hi + hi*lo, fp32 accumulate): <= 1e-4 vs the reference like WUNET_PREC_FP32 */
 #define WUNET_PREC_TF32 3   /* training step only: tf32 operands (round to nearest), fp32 accumulate on wgmma tensor cores; the
                                inference entry points reject it (WUNET_EINVAL) */
+#define WUNET_PREC_FP16 4   /* inference only: the bf16 contract with fp16 in place of bf16 — fp16 activations (channels-last) and
+                               weights (round to nearest even), fp32 accumulate on wgmma tensor cores, BatchNorm + LeakyReLU in fp32.
+                               Every fp16 store saturates: an activation beyond +-65504 is stored as +-65504, never as inf. The one
+                               place that can still overflow is the decoder's upsampling on levels of >= 128 samples, which
+                               interpolates in packed fp16 and forms b - a of two adjacent values: more than 65504 apart -> inf.
+                               Same workspace and tiling plan as WUNET_PREC_BF16; block 0 stays on the CUDA cores (WUNET_TC_ENC0
+                               does not apply). The training entry points reject it (WUNET_EINVAL). */
 
 typedef struct wunet_ctx wunet_ctx;
 
@@ -205,7 +212,7 @@ int wunet_train_backward_part(wunet_ctx *ctx, const float *x, const float *y, co
  *                    nearest, ties away from zero: cvt.rna.tf32.f32) and the products are accumulated in fp32 on wgmma
  *                    (m64nNk8.f32.tf32.tf32). This is the arithmetic of cuDNN's Conv1d with torch.backends.cudnn.allow_tf32
  *                    (PyTorch's default), i.e. of the reference's own training step on an H100. The first block stays fp32.
- *   WUNET_PREC_FP32_TC -> WUNET_EINVAL (not a training precision).
+ *   WUNET_PREC_FP32_TC, WUNET_PREC_FP16 -> WUNET_EINVAL (not training precisions).
  * The backward must use the precision and workspace of its forward. Same call sites as above (trainer/trainer.py:35-37). */
 size_t wunet_train_workspace_bytes_prec(const wunet_ctx *ctx, int B, int T, int precision);
 int wunet_train_forward_prec(wunet_ctx *ctx, const float *x, float *y, int B, int T, const float *const *conv_w,
@@ -293,8 +300,8 @@ int wunet_debug_train_layout(int n_layers, int channels_interval, int B, int T, 
  *  [23] TMA bytes per input chunk  [24] input rows used  [25] unused (0)  [26] dynamic shared memory bytes
  *  [27] threads per CTA  [28] CTAs per SM  [29] grid  [30] small (two-CTAs-per-SM) flavour  [31] tiles per frame */
 int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity);
-/* The same query for a tensor-core precision: WUNET_PREC_BF16 (= wunet_debug_plan) or WUNET_PREC_FP32_TC (the split-precision
- * plan: no row-pair form, no dense GEMM, block 0 on CUDA cores). WUNET_PREC_FP32 -> WUNET_EINVAL. */
+/* The same query for a tensor-core precision: WUNET_PREC_BF16 (= wunet_debug_plan), WUNET_PREC_FP16 (the bf16 plan) or
+ * WUNET_PREC_FP32_TC (the split-precision plan: no row-pair form, no dense GEMM, block 0 on CUDA cores). WUNET_PREC_FP32 -> WUNET_EINVAL. */
 int wunet_debug_plan_prec(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
                           int precision);
 

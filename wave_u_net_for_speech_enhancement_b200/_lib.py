@@ -11,7 +11,8 @@ PREC_FP32 = 0
 PREC_BF16 = 1
 PREC_FP32_TC = 2
 PREC_TF32 = 3
-PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC}      # inference (Model(precision=...))
+PREC_FP16 = 4
+PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC, "fp16": PREC_FP16}   # inference (Model(precision=...))
 TRAIN_PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32}      # training step (Model(train_precision=...))
 
 TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mode BatchNorm

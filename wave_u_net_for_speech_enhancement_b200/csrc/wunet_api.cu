@@ -281,6 +281,12 @@ int wunet_set_weights(wunet_ctx *c, const float *const *conv_w, const float *con
     return WUNET_OK;
 }
 
+// inference precision -> tc_* mode (0 = bf16, 1 = split precision, 2 = fp16); -1 for the fp32 path and anything else
+static int tc_mode(int precision)
+{
+    return precision == WUNET_PREC_BF16 ? 0 : precision == WUNET_PREC_FP32_TC ? 1 : precision == WUNET_PREC_FP16 ? 2 : -1;
+}
+
 size_t wunet_workspace_bytes(const wunet_ctx *c, int B, int T, int precision)
 {
     if (check_shape(c, B, T) != WUNET_OK) return 0;
@@ -290,8 +296,7 @@ size_t wunet_workspace_bytes(const wunet_ctx *c, int B, int T, int precision)
         fp32_layout(c, B, T, off, total);
         return total;
     }
-    if (precision == WUNET_PREC_BF16) return tc_workspace_bytes(c->n, c->ci, B, T, 0);
-    if (precision == WUNET_PREC_FP32_TC) return tc_workspace_bytes(c->n, c->ci, B, T, 1);
+    if (tc_mode(precision) >= 0) return tc_workspace_bytes(c->n, c->ci, B, T, tc_mode(precision));
     if (precision == WUNET_PREC_TF32) fail(WUNET_EINVAL, "WUNET_PREC_TF32 is a training precision only (the forward has no tf32 path)");
     else fail(WUNET_EINVAL, "unknown precision %d", precision);
     return 0;
@@ -312,8 +317,8 @@ int wunet_forward(wunet_ctx *c, const float *x, float *y, int B, int T, int prec
     if (precision == WUNET_PREC_FP32) return forward_fp32(c, x, y, B, T, workspace, st);
     int launches = 0;
     cudaEvent_t *ev = prof_events(c);
-    if (precision != WUNET_PREC_BF16 && precision != WUNET_PREC_FP32_TC) return fail(WUNET_EINVAL, "unknown precision %d", precision);
-    const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, precision == WUNET_PREC_FP32_TC ? 1 : 0);
+    if (tc_mode(precision) < 0) return fail(WUNET_EINVAL, "unknown precision %d", precision);
+    const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, tc_mode(precision));
     if (ev && r == 0) c->ev_recorded = 2 * c->n + 3;
     if (r != 0) return fail(WUNET_ECUDA, "tensor-core forward failed: %s", tc_error());
     c->last_launches = launches;
@@ -343,11 +348,11 @@ int wunet_forward_host(wunet_ctx *c, const float *x_host, float *y_host, int B, 
         CUDA_TRY(cudaMalloc(&c->hws, need));
         c->hws_cap = need;
     }
-    if (precision == WUNET_PREC_BF16 || precision == WUNET_PREC_FP32_TC) {
+    if (tc_mode(precision) >= 0) {
         // chunked pipeline: H2D, first/last kernels and D2H overlap per batch chunk (see tc_forward_host)
         if (!c->have_weights) return fail(WUNET_ESTATE, "wunet_forward_host called before wunet_set_weights");
         int launches = 0;
-        if (tc_forward_host(c->tc, x_host, y_host, c->hx, c->hy, B, T, c->hws, c->hstream, &launches, precision == WUNET_PREC_FP32_TC ? 1 : 0) != 0)
+        if (tc_forward_host(c->tc, x_host, y_host, c->hx, c->hy, B, T, c->hws, c->hstream, &launches, tc_mode(precision)) != 0)
             return fail(WUNET_ECUDA, "tensor-core host pipeline failed: %s", tc_error());
         c->last_launches = launches;
         return WUNET_OK;
@@ -445,8 +450,8 @@ int wunet_read_level(wunet_ctx *c, int block, const void *workspace, int B, int 
                                  (size_t)B * c->blocks[block].cout * L * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return WUNET_OK;
     }
-    if (precision == WUNET_PREC_BF16 || precision == WUNET_PREC_FP32_TC) {
-        const int r = tc_read_level(c->tc, block, workspace, B, T, out_dev, st, precision == WUNET_PREC_FP32_TC ? 1 : 0);
+    if (tc_mode(precision) >= 0) {
+        const int r = tc_read_level(c->tc, block, workspace, B, T, out_dev, st, tc_mode(precision));
         if (r != 0) return fail(WUNET_ECUDA, "tc_read_level failed: %s", tc_error());
         return WUNET_OK;
     }
@@ -461,9 +466,9 @@ static int train_prec(int precision)
     if (precision == WUNET_PREC_FP32) return TRAIN_FP32;
     if (precision == WUNET_PREC_BF16) return TRAIN_BF16;
     if (precision == WUNET_PREC_TF32) return TRAIN_TF32;
-    if (precision == WUNET_PREC_FP32_TC)
-        fail(WUNET_EINVAL, "training precision WUNET_PREC_FP32_TC is not supported: use WUNET_PREC_FP32, WUNET_PREC_BF16 or "
-                           "WUNET_PREC_TF32");
+    if (precision == WUNET_PREC_FP32_TC || precision == WUNET_PREC_FP16)
+        fail(WUNET_EINVAL, "training precision %s is not supported: use WUNET_PREC_FP32, WUNET_PREC_BF16 or WUNET_PREC_TF32",
+             precision == WUNET_PREC_FP16 ? "WUNET_PREC_FP16" : "WUNET_PREC_FP32_TC");
     else
         fail(WUNET_EINVAL, "unknown training precision %d", precision);
     return -1;
@@ -636,15 +641,14 @@ int wunet_debug_plan_prec(int n_layers, int channels_interval, int B, int T, int
 {
     if (n_layers < 1 || n_layers > 16 || channels_interval < 1 || B < 1 || T < 1 || (T % (1 << n_layers)) != 0 || num_sms < 1)
         return fail(WUNET_EINVAL, "bad plan query");
-    if (precision != WUNET_PREC_BF16 && precision != WUNET_PREC_FP32_TC)
-        return fail(WUNET_EINVAL, "only the tensor-core precisions (bf16, fp32_tc) have a tiling plan");
+    if (tc_mode(precision) < 0) return fail(WUNET_EINVAL, "only the tensor-core precisions (bf16, fp32_tc, fp16) have a tiling plan");
     const int n = n_layers, ci = channels_interval;
     std::vector<TcBlockSrc> src;            // same channel plan as wunet_create (model/unet_basic.py:38-39, :52-57, :59-62)
     for (int i = 0; i < n; ++i) src.push_back(TcBlockSrc{i == 0 ? 1 : i * ci, (i + 1) * ci, 15, nullptr, nullptr, nullptr});
     src.push_back(TcBlockSrc{n * ci, n * ci, 15, nullptr, nullptr, nullptr});
     for (int j = 0; j < n; ++j)
         src.push_back(TcBlockSrc{j == 0 ? 2 * n * ci : (2 * (n - j) + 1) * ci, (n - j) * ci, 5, nullptr, nullptr, nullptr});
-    if (tc_debug_plan(n, ci, src.data(), (int)src.size(), B, T, block, num_sms, fields, capacity, precision == WUNET_PREC_FP32_TC ? 1 : 0))
+    if (tc_debug_plan(n, ci, src.data(), (int)src.size(), B, T, block, num_sms, fields, capacity, tc_mode(precision)))
         return fail(WUNET_EINVAL, "%s", tc_error());
     return WUNET_OK;
 }

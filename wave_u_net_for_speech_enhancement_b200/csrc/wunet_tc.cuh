@@ -1,4 +1,4 @@
-// wunet_tc.cuh — interface of the bf16 / wgmma tensor-core path (implemented in wunet_tc.cu).
+// wunet_tc.cuh — interface of the bf16 / fp16 / wgmma tensor-core path (implemented in wunet_tc.cu and wunet_tc_f16.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -19,7 +19,8 @@ struct TcBlockSrc {
 const char *tc_error();
 int tc_set_weights(TcState **st, int n_layers, int ci, const TcBlockSrc *blocks, int nblocks, const float *out_w,
                    const float *out_b, cudaStream_t stream);
-// mode: 0 = bf16 activations; 1 = split precision (fp32_tc): activations as [hi | lo] bf16 halves, three MMAs per product
+// mode: 0 = bf16 activations; 1 = split precision (fp32_tc): activations as [hi | lo] bf16 halves, three MMAs per product;
+// 2 = fp16 activations and weights (the bf16 layout and plan; the fp16 weights are packed by the first fp16 forward)
 size_t tc_workspace_bytes(int n_layers, int ci, int B, int T, int mode = 0);
 // events: null, or 2n+3 events: [0] before the first kernel, [i+1] after block i, [2n+2] after the head
 int tc_forward(TcState *st, const float *x, float *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
@@ -30,7 +31,7 @@ int tc_forward_host(TcState *st, const float *x_host, float *y_host, float *x_de
 int tc_read_level(TcState *st, int block, const void *ws, int B, int T, float *out_ncl, cudaStream_t stream, int mode = 0);
 void tc_destroy(TcState *st);
 // host-only: the tiling build_plan would choose for `block` (32 ints, see wunet_debug_plan in include/wunet_b200.h); mode 1 =
-// the split-precision (fp32_tc) plan
+// the split-precision (fp32_tc) plan; mode 2 (fp16) = the bf16 plan
 int tc_debug_plan(int n_layers, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *fields,
                   int capacity, int mode = 0);
 

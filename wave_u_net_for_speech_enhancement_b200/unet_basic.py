@@ -227,7 +227,11 @@ class Model(nn.Module):
     precision      "fp32_tc" (default): fp32-grade results on the tensor cores (bf16 hi + lo split, three MMAs per
                    product; <=1e-4 vs the reference, measured 1e-6; needs channels_interval % 8 == 0 and <= 32);
                    "fp32": the same contract on CUDA-core FFMA for any channel plan (slower);
-                   "bf16": bf16 activations / operands on the tensor cores (the fastest path; ~6e-4 on the output).
+                   "bf16": bf16 activations / operands on the tensor cores (the fastest path; ~6e-4 on the output);
+                   "fp16": the bf16 contract with fp16 activations / operands (11-bit significand, the precision of the
+                   TF32 convolutions cuDNN runs for the reference on an H100) at bf16's speed. fp16 stores saturate at
+                   +-65504; activations near that range are not what this model produces. Same channel-plan needs as
+                   "fp32_tc". Inference only: ``train_precision`` does not accept it.
     train_backend  "native" (default): a forward in training mode runs ``wunet_train_forward`` (BatchNorm with batch
                    statistics, running buffers updated) behind a ``torch.autograd.Function`` whose backward is
                    ``wunet_train_backward_part``; the reference's loss, ``loss.backward()`` and optimizer run unchanged
