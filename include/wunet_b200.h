@@ -262,6 +262,30 @@ int wunet_train_backward_ex(wunet_ctx *ctx, const float *x, const float *y, cons
                             const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
                             float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                             void *stream, float *dx, int part, int precision, int flags);
+/* BatchNorm statistics synchronised over data-parallel ranks: what nn.SyncBatchNorm (torch.nn.SyncBatchNorm.
+ * convert_sync_batchnorm(model)) computes in a one-process-per-GPU step. With a hook installed, every training forward with
+ * batch statistics (not WUNET_TRAIN_FROZEN_BN) on this context, and its backward, compute the BatchNorm reductions from sums
+ * over every rank's frames:
+ *   forward, per block (C = its Cout, N = sum over ranks of B L): mean = sum z / N and var = sum (z - mean)^2 / N (a second
+ *     pass about the GLOBAL mean), both in double and rounded to fp32 as without the hook; the running statistics use var
+ *     N / (N - 1) and come out identical on every rank;
+ *   backward: mean(dy) and mean(dy zhat) over the N values; the BatchNorm weight / bias gradients stay this rank's sums (the
+ *     caller's gradient all-reduce averages them: nn.SyncBatchNorm + DistributedDataParallel arithmetic).
+ * `fn` is called on the calling host thread, after the kernels that wrote buf[0 .. count) are enqueued on the call's `stream`;
+ * it must leave the element-wise SUM over ranks in buf[0 .. count), ordered on `stream` (an NCCL all-reduce on that stream
+ * does this). A nonzero return fails the call with WUNET_ECUDA naming the block; nothing after that point is enqueued.
+ * Calls per block, in order:
+ *   forward pass 1: buf[0 .. C) = local sum z, buf[C] = local B L                  -> fn(user, buf, C + 1, stream)
+ *   forward pass 2: buf[C + 1 .. 2C + 1) = local sum (z - mean)^2                  -> fn(user, buf + C + 1, C, stream)
+ *   backward, each block of the part in processing order: [sum dy | sum dy zhat | B L] -> fn(user, buf, 2C + 1, stream)
+ * buf: caller-owned device memory of at least 2 * n_layers * channels_interval + 1 doubles (smaller -> WUNET_EINVAL), alive
+ * while the hook is installed. fn == NULL uninstalls the hook (the default: per-rank statistics, exactly the launches of a
+ * context that never had one). The one-value-per-channel check of wunet_train_forward_ex does not apply to a synchronised
+ * forward (nn.SyncBatchNorm raises only without other ranks). A forward and its backward must agree on the hook being
+ * installed. No reference counterpart: the reference's nn.DataParallel replicas keep per-replica statistics. */
+typedef int (*wunet_bn_allreduce_fn)(void *user, double *buf, size_t count, void *stream);
+int wunet_train_set_bn_allreduce(wunet_ctx *ctx, wunet_bn_allreduce_fn fn, void *user, double *buf, size_t capacity);
+
 /* Test hook, synchronous, on caller device buffers (fp32): one convolution-shaped pass of the training step at `precision`
  * (WUNET_PREC_FP32, WUNET_PREC_BF16 or WUNET_PREC_TF32), the kernels the step itself uses. mode: 0 = direct, 1 = decimated (src0 is
  * [B][cin0][2L], every other sample read), 2 = upsample + concat (src0 = [B][cin0][L/2] interpolated 2x linearly,

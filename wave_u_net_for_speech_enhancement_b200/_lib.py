@@ -19,6 +19,9 @@ TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mo
 TRAIN_NO_PARAM_GRADS = 2   # backward: input gradient only
 TRAIN_DETERMINISTIC = 16   # bitwise repeatable step (no float atomics; larger workspace)
 
+# wunet_bn_allreduce_fn(user, buf, count, stream): sums buf[0 .. count) (device doubles) over the ranks, ordered on stream
+BN_ALLREDUCE_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p)
+
 _lib = None
 
 
@@ -78,6 +81,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_backward_part_prec.argtypes = lib.wunet_train_backward_part.argtypes + [ci]
     lib.wunet_train_forward_ex.argtypes = lib.wunet_train_forward_prec.argtypes + [ci]
     lib.wunet_train_backward_ex.argtypes = lib.wunet_train_backward.argtypes + [vp, ci, ci, ci]
+    lib.wunet_train_set_bn_allreduce.argtypes = [vp, BN_ALLREDUCE_FN, vp, vp, cs]
     lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     lib.wunet_debug_train_layout.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ll), ci]
     _lib = lib
@@ -97,6 +101,7 @@ EXPORTED_SYMBOLS = [
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
     "wunet_train_forward_ex", "wunet_train_backward_ex", "wunet_train_workspace_bytes_ex", "wunet_debug_train_layout",
+    "wunet_train_set_bn_allreduce",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]

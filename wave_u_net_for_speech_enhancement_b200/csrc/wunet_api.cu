@@ -69,6 +69,8 @@ struct wunet_ctx {
     cudaEvent_t e_in[2] = {}, e_comp[2] = {}, e_done[2] = {};
     bool slot_busy[2] = {false, false};
     int next_ticket = 0;
+    // BatchNorm all-reduce hook of the training step (wunet_train_set_bn_allreduce); fn == nullptr: per-rank statistics
+    BnSync bn_sync{nullptr, nullptr, nullptr};
 };
 
 namespace {
@@ -537,8 +539,10 @@ int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T,
     if (prec < 0) return WUNET_EINVAL;
     if (flags & ~kTrainFlags) return fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
     // batch statistics of one value per channel (B = 1 and L = 1 at the middle block): torch.nn.BatchNorm1d raises in training
-    // mode rather than normalise by a variance of 0
-    if (!(flags & WUNET_TRAIN_FROZEN_BN) && B == 1 && (T >> c->n) == 1)
+    // mode rather than normalise by a variance of 0. Synchronised statistics count every rank's frames (nn.SyncBatchNorm
+    // raises only without other ranks).
+    const bool synced = c->bn_sync.fn && !(flags & WUNET_TRAIN_FROZEN_BN);
+    if (!(flags & WUNET_TRAIN_FROZEN_BN) && !synced && B == 1 && (T >> c->n) == 1)
         return fail(WUNET_EINVAL, "Expected more than 1 value per channel when training (B=1, T=%d: one value per channel at the "
                                   "middle block)", T);
     if (!x || !y || !workspace || !conv_w || !conv_b || !bn_weight || !bn_bias || !bn_running_mean || !bn_running_var || !out_w || !out_b)
@@ -548,7 +552,8 @@ int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T,
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b};
-    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec, tflags))
+    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec, tflags,
+                      synced ? &c->bn_sync : nullptr))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
 }
@@ -604,8 +609,24 @@ int wunet_train_backward_ex(wunet_ctx *c, const float *x, const float *y, const 
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, nullptr, bn_weight, bn_bias, nullptr, nullptr, out_w, nullptr};
     const TrainGrads G{g_conv_w, g_conv_b, g_bn_weight, g_bn_bias, g_out_w, g_out_b};
-    if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec, dx, tflags))
+    const bool synced = c->bn_sync.fn && !(flags & WUNET_TRAIN_FROZEN_BN);
+    if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec, dx, tflags,
+                       synced ? &c->bn_sync : nullptr))
         return fail(WUNET_ECUDA, "%s", train_error());
+    return WUNET_OK;
+}
+
+int wunet_train_set_bn_allreduce(wunet_ctx *c, wunet_bn_allreduce_fn fn, void *user, double *buf, size_t capacity)
+{
+    if (!c) return fail(WUNET_EINVAL, "null context");
+    if (!fn) {
+        c->bn_sync = BnSync{nullptr, nullptr, nullptr};
+        return WUNET_OK;
+    }
+    const size_t need = 2 * (size_t)c->n * c->ci + 1;                 // [sum dy | sum dy zh | B L] of the widest block (n ci)
+    if (!buf || capacity < need)
+        return fail(WUNET_EINVAL, "BatchNorm all-reduce buffer too small: %zu < %zu doubles", buf ? capacity : (size_t)0, need);
+    c->bn_sync = BnSync{fn, user, buf};
     return WUNET_OK;
 }
 

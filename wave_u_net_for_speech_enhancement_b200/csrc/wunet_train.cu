@@ -16,6 +16,8 @@
 // TRAIN_FROZEN_BN (eval-mode BatchNorm: running statistics, never updated) and TRAIN_NO_PARAM_GRADS (input gradient only) only
 // change the BatchNorm arithmetic and which reductions run; the convolution-shaped passes are the same kernels. The input
 // gradient dx is train_input_grad_kernel below (head's raw-input channel + block 0's transposed conv).
+// BnSync (nn.SyncBatchNorm over data-parallel ranks): the batch-statistics reductions are split at the cross-rank sums
+// (train_bn_sync_* kernels, a host hook between them); without it the step issues exactly the launches it always did.
 //
 // Reference: trainer/trainer.py:34-38 (forward, loss.backward()), model/unet_basic.py:77-100 with the BatchNorm1d of
 // :12, :25, :55 in .train() mode (batch statistics; running statistics updated with momentum 0.1 and the unbiased variance).
@@ -121,6 +123,63 @@ __global__ void __launch_bounds__(256) train_bn_stats_kernel(const float *__rest
         running_mean[c] = (float)((1.0 - momentum) * (double)running_mean[c] + momentum * mu);
         running_var[c] = (float)((1.0 - momentum) * (double)running_var[c] + momentum * unbiased);
     }
+}
+
+// The same statistics synchronised over data-parallel ranks (nn.SyncBatchNorm; BnSync), split where the cross-rank sums go.
+// Each pass has train_bn_stats_kernel's loop and block_sum order, so a pass-through hook reproduces it bit for bit.
+// pass 1: buf[c] = local sum z, buf[C] = local B L                                  -> hook(buf, C + 1)
+__global__ void __launch_bounds__(256) train_bn_sync_sum_kernel(const float *__restrict__ z, int B, int C, int L,
+                                                                double *__restrict__ buf)
+{
+    __shared__ double sh[8];
+    const int c = blockIdx.x;
+    const long long n = (long long)B * L;
+    double s = 0.0;
+    for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+        const int b = (int)(i / L), l = (int)(i - (long long)b * L);
+        s += (double)z[((size_t)b * C + c) * L + l];
+    }
+    const double t = block_sum(s, sh);
+    if (threadIdx.x == 0) {
+        buf[c] = t;
+        if (c == 0) buf[C] = (double)n;
+    }
+}
+
+// pass 2: buf[C + 1 + c] = local sum (z - mean)^2 about the global mean buf[c] / buf[C]        -> hook(buf + C + 1, C)
+__global__ void __launch_bounds__(256) train_bn_sync_centred_kernel(const float *__restrict__ z, int B, int C, int L,
+                                                                    double *__restrict__ buf)
+{
+    __shared__ double sh[8];
+    const int c = blockIdx.x;
+    const long long n = (long long)B * L;
+    const double mu = buf[c] / buf[C];
+    double q = 0.0;
+    for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+        const int b = (int)(i / L), l = (int)(i - (long long)b * L);
+        const double d = (double)z[((size_t)b * C + c) * L + l] - mu;
+        q += d * d;
+    }
+    const double t = block_sum(q, sh);
+    if (threadIdx.x == 0) buf[C + 1 + c] = t;
+}
+
+// mean, invstd and the running statistics from the global sums, rounded as train_bn_stats_kernel rounds them
+__global__ void train_bn_sync_finalize_kernel(const double *__restrict__ buf, int C, float momentum, float *__restrict__ mean,
+                                              float *__restrict__ invstd, float *__restrict__ running_mean,
+                                              float *__restrict__ running_var)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    const double nd = buf[C];
+    const long long n = (long long)nd;
+    const double mu = buf[c] / nd;
+    const double var = buf[C + 1 + c] / nd;
+    mean[c] = (float)mu;
+    invstd[c] = (float)(1.0 / sqrt(var + (double)kBnEps));
+    const double unbiased = var * ((double)n / (double)(n > 1 ? n - 1 : 1));
+    running_mean[c] = (float)((1.0 - momentum) * (double)running_mean[c] + momentum * mu);
+    running_var[c] = (float)((1.0 - momentum) * (double)running_var[c] + momentum * unbiased);
 }
 
 // eval-mode BatchNorm (TRAIN_FROZEN_BN, model/unet_basic.py in .eval()): normalise by the running statistics, rounding invstd
@@ -258,6 +317,50 @@ __global__ void __launch_bounds__(256) train_bn_bwd_stats_kernel(const float *__
         s1[c] = (float)(t1 / (double)n);                        // mean(dy), mean(dy zh): what the input gradient needs
         s2[c] = (float)(t2 / (double)n);
     }
+}
+
+// The same reductions synchronised over data-parallel ranks (BnSync), train_bn_bwd_stats_kernel's loop and block_sum order:
+// g_beta, g_gamma get the LOCAL sums (the gradient all-reduce averages them, as with nn.SyncBatchNorm under DDP);
+// buf = [sum dy | sum dy zh | B L] (2C + 1)                                            -> hook(buf, 2C + 1)
+__global__ void __launch_bounds__(256) train_bn_sync_bwd_sums_kernel(const float *__restrict__ ga, const float *__restrict__ z,
+                                                                     const float *__restrict__ mean, const float *__restrict__ invstd,
+                                                                     const float *__restrict__ gamma, const float *__restrict__ beta,
+                                                                     float *__restrict__ g_gamma, float *__restrict__ g_beta,
+                                                                     double *__restrict__ buf, int B, int C, int L)
+{
+    __shared__ double sh[8];
+    const int c = blockIdx.x;
+    const long long n = (long long)B * L;
+    const float mu = mean[c], is = invstd[c], g = gamma[c], be = beta[c];
+    double a1 = 0.0, a2 = 0.0;
+    for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+        const int b = (int)(i / L), l = (int)(i - (long long)b * L);
+        const size_t idx = ((size_t)b * C + c) * L + l;
+        const float zh = (z[idx] - mu) * is;
+        const float yv = fmaf(g, zh, be);
+        const float dyv = yv >= 0.f ? ga[idx] : kLreluSlope * ga[idx];
+        a1 += (double)dyv;
+        a2 += (double)dyv * (double)zh;
+    }
+    const double t1 = block_sum(a1, sh);
+    const double t2 = block_sum(a2, sh);
+    if (threadIdx.x == 0) {
+        if (g_beta) g_beta[c] = (float)t1;                     // null under TRAIN_NO_PARAM_GRADS
+        if (g_gamma) g_gamma[c] = (float)t2;
+        buf[c] = t1;
+        buf[C + c] = t2;
+        if (c == 0) buf[2 * C] = (double)n;
+    }
+}
+
+// s1 = mean(dy), s2 = mean(dy zh) over every rank's frames, from the global sums
+__global__ void train_bn_sync_bwd_finalize_kernel(const double *__restrict__ buf, int C, float *__restrict__ s1,
+                                                  float *__restrict__ s2)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    s1[c] = (float)(buf[c] / buf[2 * C]);
+    s2[c] = (float)(buf[C + c] / buf[2 * C]);
 }
 
 //   dz = invstd gamma (dy - mean(dy) - zh mean(dy zh))      written over ga (in place)
@@ -734,9 +837,10 @@ size_t train_workspace_bytes(int n, int ci, int B, int T, int prec, int flags)
 }
 
 int train_forward(int n, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum, void *workspace,
-                  cudaStream_t st, int prec, int flags)
+                  cudaStream_t st, int prec, int flags, const BnSync *sync)
 {
     const bool frozen = flags & TRAIN_FROZEN_BN;
+    if (frozen) sync = nullptr;                                     // running statistics: nothing to synchronise
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
@@ -777,7 +881,17 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
         if (frozen)
             train_bn_frozen_stats_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(P.bn_mean[i], P.bn_var[i], ws + lo.mean[i],
                                                                                    ws + lo.invstd[i], s.cout);
-        else
+        else if (sync) {
+            double *buf = sync->buf;
+            train_bn_sync_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, buf);
+            if (const int rc = sync->fn(sync->user, buf, (size_t)s.cout + 1, st))
+                return train_fail("training forward, block %d: the BatchNorm all-reduce hook failed on the sums (status %d)", i, rc);
+            train_bn_sync_centred_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, buf);
+            if (const int rc = sync->fn(sync->user, buf + s.cout + 1, (size_t)s.cout, st))
+                return train_fail("training forward, block %d: the BatchNorm all-reduce hook failed on the variances (status %d)", i, rc);
+            train_bn_sync_finalize_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(buf, s.cout, momentum, ws + lo.mean[i], ws + lo.invstd[i],
+                                                                                    P.bn_mean[i], P.bn_var[i]);
+        } else
             train_bn_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, momentum, ws + lo.mean[i], ws + lo.invstd[i],
                                                                      P.bn_mean[i], P.bn_var[i]);
         const long long nel = (long long)B * s.cout * s.L;
@@ -792,7 +906,8 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
 }
 
 int train_backward(int n, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
-                   const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec, float *dx, int flags)
+                   const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec, float *dx, int flags,
+                   const BnSync *sync)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
@@ -802,6 +917,7 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
     const int last = 2 * n, C = sh[last].cout;
     const bool naive = train_naive() && prec == TRAIN_FP32;
     const bool frozen = flags & TRAIN_FROZEN_BN, pgrads = !(flags & TRAIN_NO_PARAM_GRADS);
+    if (frozen) sync = nullptr;                                     // as in the forward
     const bool det = pgrads && (flags & TRAIN_DETERMINISTIC);      // without parameter gradients nothing is summed atomically
     float *scratch = ws + lo.total;                                 // TRAIN_DETERMINISTIC only (det_scratch_floats)
     if (part < -1 || part > 1) return train_fail("training backward: part must be -1, 0 or 1 (got %d)", part);
@@ -831,7 +947,14 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         const long long nel = (long long)B * s.cout * s.L;
         // batch statistics: dz needs mean(dy) and mean(dy zh) (s1, s2); frozen statistics: they are constants, dz = invstd
         // gamma dy (s1 = s2 = 0), and the reductions only serve the BatchNorm parameter gradients
-        if (!frozen || pgrads)
+        if (sync) {
+            train_bn_sync_bwd_sums_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i],
+                                                                             P.bn_b[i], pgrads ? G.bn_w[i] : nullptr,
+                                                                             pgrads ? G.bn_b[i] : nullptr, sync->buf, B, s.cout, s.L);
+            if (const int rc = sync->fn(sync->user, sync->buf, 2 * (size_t)s.cout + 1, st))
+                return train_fail("training backward, block %d: the BatchNorm all-reduce hook failed (status %d)", i, rc);
+            train_bn_sync_bwd_finalize_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(sync->buf, s.cout, ws + lo.s1[i], ws + lo.s2[i]);
+        } else if (!frozen || pgrads)
             train_bn_bwd_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
                                                                          pgrads ? G.bn_w[i] : nullptr, pgrads ? G.bn_b[i] : nullptr,
                                                                          ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);

@@ -35,19 +35,31 @@ enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1, TRAIN_TF32 = 2 };
 // step must agree on it.
 enum TrainFlags : int { TRAIN_FROZEN_BN = 1, TRAIN_NO_PARAM_GRADS = 2, TRAIN_DETERMINISTIC = 4 };
 
+// BatchNorm statistics synchronised over data-parallel ranks (nn.SyncBatchNorm; wunet_train_set_bn_allreduce): the batch
+// statistics and the backward's mean(dy), mean(dy zh) are computed from sums over every rank's frames. `fn` is called on the
+// host after the kernels that wrote buf[0 .. count) are enqueued on `stream`, and must leave the element-wise sum over ranks
+// there, ordered on `stream`; nonzero = failure. buf holds >= 2 Cout + 1 doubles of the widest block (device memory).
+struct BnSync {
+    int (*fn)(void *user, double *buf, size_t count, void *stream);
+    void *user;
+    double *buf;
+};
+
 const char *train_error();
 size_t train_workspace_bytes(int n_layers, int ci, int B, int T, int prec = TRAIN_FP32, int flags = 0);
 // y = model(x) with BatchNorm in training mode (or, with TRAIN_FROZEN_BN, eval mode); keeps every pre-BN output and
-// activation in `workspace` for the backward
+// activation in `workspace` for the backward. sync (batch statistics only; null = this rank's frames alone): per block,
+// the local sum z and B L, hook, the local sum (z - global mean)^2, hook.
 int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum,
-                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32, int flags = 0);
+                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32, int flags = 0, const BnSync *sync = nullptr);
 // gradients of every parameter for the upstream gradient dy of the output; `workspace` as left by train_forward.
 // part: -1 = the whole backward; 0 = head + decoder blocks (their gradients are complete afterwards: a data-parallel caller
 // starts reducing them while part 1 runs); 1 = middle + encoder blocks (must follow part 0 on the same stream).
 // dx (optional, [B][1][T], fully overwritten): gradient of the input x; written by part -1 or 1 (block 0 is in part 1).
+// sync: must be given iff the forward had it; per block of the part, [sum dy | sum dy zh | B L], hook.
 int train_backward(int n_layers, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
                    const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1, int prec = TRAIN_FP32,
-                   float *dx = nullptr, int flags = 0);
+                   float *dx = nullptr, int flags = 0, const BnSync *sync = nullptr);
 // One convolution-shaped pass on caller device buffers (test hook): pass 0 = forward conv out[B][Cout][L] = conv(in, w);
 // 1 = input gradient out[B][Cin][L] of dz [B][Cout][L] (Conv1d padding, no mode); 2 = weight gradient out[Cout][Cin][K] =
 // sum dz * in. `in` is built from src0 / src1 per `mode` as in the forward (ConvArgs). Synchronous.

@@ -5,8 +5,10 @@ the batch, replicates the parameters, runs per-replica forwards (BatchNorm stati
 gradients on GPU 0. Here it is one process per GPU: each rank steps its own shard of the batch and the gradients are
 averaged over ONE flat bucket (NCCL on GPUs, gloo in the CPU tests) before the caller's unchanged optimizer step — the mean
 over ranks of per-shard mean losses is the reference's mean loss over the whole batch when the shards are equal. BatchNorm
-running statistics stay per rank, as they stay per replica in the reference (only replica 0's survive there; rank 0 writes
-the checkpoint here).
+statistics stay per rank, as they stay per replica in the reference (only replica 0's survive there; rank 0 writes the
+checkpoint here), unless the model is converted with ``nn.SyncBatchNorm.convert_sync_batchnorm``: the native step then
+computes them over every rank's frames (three small all-reduces per block, on the current stream), and with equal shards the
+averaged step equals the single-process step on the concatenated batch.
 
 The bucket is laid out in the order the backward pass FINISHES the gradients (head, decoder blocks last to first, middle,
 encoder blocks last to first) and cut in two parts at the decoder / middle boundary: the native backward

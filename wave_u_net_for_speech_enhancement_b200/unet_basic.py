@@ -26,6 +26,7 @@ import threading
 from typing import Dict, Optional, Tuple
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 
 from . import _lib
@@ -130,6 +131,36 @@ class _NativeState:
             pass
 
 
+def _native_call(lib, c, reducer, buf, call):
+    """``call()`` (a training entry point, returning its status) with, when ``reducer`` is set, the BatchNorm all-reduce hook
+    installed around it (wunet_train_set_bn_allreduce): the hook hands ``reducer`` the float64 view of ``buf`` the library
+    names, to be summed over the ranks in place on the current stream. An exception raised in the reducer fails the call and
+    is re-raised here; the hook is uninstalled in every case."""
+    if reducer is None:
+        _lib.check(call())
+        return
+    errors = []
+
+    def hook(user, ptr, count, stream):
+        try:
+            off = (ptr - buf.data_ptr()) // buf.element_size()
+            reducer(buf[off:off + count])
+            return 0
+        except BaseException as e:  # noqa: BLE001 - re-raised after the C call
+            errors.append(e)
+            return 1
+
+    fn = _lib.BN_ALLREDUCE_FN(hook)                      # kept alive for the whole call
+    _lib.check(lib.wunet_train_set_bn_allreduce(c, fn, None, buf.data_ptr(), buf.numel()))
+    try:
+        rc = call()
+    finally:
+        lib.wunet_train_set_bn_allreduce(c, _lib.BN_ALLREDUCE_FN(), None, None, 0)     # a null fn uninstalls
+    if errors:
+        raise errors[0]
+    _lib.check(rc)
+
+
 class _NativeTrainStep(torch.autograd.Function):
     """forward = wunet_train_forward_ex, backward = wunet_train_backward_ex (include/wunet_b200.h). The activations live in a
     workspace tensor kept on the autograd context; parameter order: 4 per conv block (conv.weight, conv.bias, bn.weight,
@@ -139,14 +170,17 @@ class _NativeTrainStep(torch.autograd.Function):
     normalising by the running statistics, which stay untouched (.eval()); either may add ``_lib.TRAIN_DETERMINISTIC`` (weight
     and head gradients summed in a fixed order, with a larger workspace). The backward fills the gradient of ``x`` when it
     requires grad and those of the parameters when any of them does; with no parameter requiring grad it computes ``dx``
-    only (no weight-gradient pass, no reduction, no all-reduce)."""
+    only (no weight-gradient pass, no reduction, no all-reduce).
+
+    ``reducer``: None, or the callable that sums a float64 CUDA view over the data-parallel ranks in place (nn.SyncBatchNorm):
+    the forward's batch statistics and its backward's BatchNorm means then cover every rank's frames."""
 
     @staticmethod
     def _ptr_array(tensors):
         return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
 
     @staticmethod
-    def forward(ctx, model, flags, x, *params):
+    def forward(ctx, model, flags, reducer, x, *params):
         lib = _lib.load()
         blocks = model._blocks()
         nb = len(blocks)
@@ -168,12 +202,16 @@ class _NativeTrainStep(torch.autograd.Function):
             momentum = float(blocks[0][1].momentum)
             stream = torch.cuda.current_stream(x.device).cuda_stream
             P = _NativeTrainStep._ptr_array
-            _lib.check(lib.wunet_train_forward_ex(c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b),
-                                                  P(rmean), P(rvar), params[-2].data_ptr(), params[-1].data_ptr(), momentum,
-                                                  ws.data_ptr(), ws.numel(), stream, prec, flags))
-        # the backward runs at the precision and BatchNorm mode of ITS forward (and reads the bf16 weight packings that
-        # forward left in ws)
+            # [sum dy | sum dy zhat | B L] of the widest block (n ci channels): the hook's exchange buffer
+            bn_buf = None if reducer is None else torch.empty(2 * model.n_layers * model.channels_interval + 1,
+                                                              dtype=torch.float64, device=x.device)
+            _native_call(lib, c, reducer, bn_buf, lambda: lib.wunet_train_forward_ex(
+                c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b), P(rmean), P(rvar),
+                params[-2].data_ptr(), params[-1].data_ptr(), momentum, ws.data_ptr(), ws.numel(), stream, prec, flags))
+        # the backward runs at the precision, BatchNorm mode and synchronisation of ITS forward (and reads the bf16 weight
+        # packings that forward left in ws)
         ctx.model, ctx.ws, ctx.nb, ctx.prec, ctx.flags = model, ws, nb, prec, flags
+        ctx.reducer, ctx.bn_buf = reducer, bn_buf
         ctx.save_for_backward(x, y, *params)
         return y
 
@@ -185,8 +223,8 @@ class _NativeTrainStep(torch.autograd.Function):
         nb = ctx.nb
         B, _, T = x.shape
         gy = gy.contiguous()
-        want_dx = ctx.needs_input_grad[2]
-        want_params = any(ctx.needs_input_grad[3:])
+        want_dx = ctx.needs_input_grad[3]
+        want_params = any(ctx.needs_input_grad[4:])
         dx = torch.empty_like(x) if want_dx else None
         flags = ctx.flags | (0 if want_params else _lib.TRAIN_NO_PARAM_GRADS)
         if want_params:
@@ -205,18 +243,17 @@ class _NativeTrainStep(torch.autograd.Function):
             G = (lambda k: P(sel(grads, k))) if want_params else (lambda k: None)   # noqa: E731
             ptr = lambda t: None if t is None else t.data_ptr()               # noqa: E731
             for part in ((0, 1) if reduce else (-1,)):
-                _lib.check(lib.wunet_train_backward_ex(c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)),
-                                                       P(sel(params, 2)), P(sel(params, 3)), params[-2].data_ptr(),
-                                                       G(0), G(1), G(2), G(3), ptr(grads[-2]), ptr(grads[-1]), ctx.ws.data_ptr(),
-                                                       ctx.ws.numel(), stream, ptr(dx) if part != 0 else None, part, ctx.prec,
-                                                       flags))
+                _native_call(lib, c, ctx.reducer, ctx.bn_buf, lambda: lib.wunet_train_backward_ex(
+                    c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)), P(sel(params, 2)), P(sel(params, 3)),
+                    params[-2].data_ptr(), G(0), G(1), G(2), G(3), ptr(grads[-2]), ptr(grads[-1]), ctx.ws.data_ptr(),
+                    ctx.ws.numel(), stream, ptr(dx) if part != 0 else None, part, ctx.prec, flags))
                 if reduce:
                     # head + decoder gradients are final after part 0: their all-reduce overlaps part 1 (middle + encoders)
                     bucket.reduce_part(part)
             if reduce:
                 bucket.finish()
-        ctx.ws = None
-        return (None, None, dx, *grads)                      # no gradient for the model handle and the flags
+        ctx.ws = ctx.bn_buf = ctx.reducer = None
+        return (None, None, None, dx, *grads)                # no gradient for the model handle, the flags and the reducer
 
 
 class Model(nn.Module):
@@ -272,6 +309,12 @@ class Model(nn.Module):
     training workspace (about 70 MB in fp32, 22 MB in bf16 at the reference's batch of 120 x 16384). Note that
     ``torch.use_deterministic_algorithms(True)`` also makes torch fill every ``torch.empty`` tensor, including the training
     workspace, on every step (``torch.utils.deterministic.fill_uninitialized_memory``); that setting is left to the caller.
+
+    Synchronised BatchNorm (no constructor argument): after ``nn.SyncBatchNorm.convert_sync_batchnorm(model)`` a native
+    training forward with batch statistics, and its backward, compute the BatchNorm statistics over every rank's frames when
+    ``torch.distributed`` is initialised and the containers' process group has more than one rank, as ``nn.SyncBatchNorm``
+    does (three small all-reduces per block, on the current stream). The running statistics then agree on every rank, and
+    with equal shards the data-parallel step equals the single-process step on the concatenated batch.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
@@ -310,6 +353,9 @@ class Model(nn.Module):
 
         # native state (not part of state_dict); shared by reference with DataParallel replicas, see _NativeState
         self._native = _NativeState()
+        # private seam: a callable summing a float64 CUDA view over the ranks in place forces the synchronised BatchNorm path
+        # (see _bn_sync_reducer)
+        self._bn_allreduce = None
 
     # ------------------------------------------------------------------------------------------
     # native plumbing
@@ -416,7 +462,8 @@ class Model(nn.Module):
         ``train_precision="bf16"`` / ``"tf32"``, bf16 / tf32 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
         B, _, T = x.shape
-        if not frozen_bn and B * (T >> self.n_layers) == 1:
+        reducer = None if frozen_bn else self._bn_sync_reducer()
+        if not frozen_bn and reducer is None and B * (T >> self.n_layers) == 1:
             # torch.nn.BatchNorm1d in training mode refuses batch statistics of one value per channel (here: the middle
             # block of a single frame of 2^n_layers samples); the reference raises this from self.middle
             raise ValueError("Expected more than 1 value per channel when training, got input size "
@@ -435,7 +482,7 @@ class Model(nn.Module):
         flags = _lib.TRAIN_FROZEN_BN if frozen_bn else 0
         if torch.backends.cudnn.deterministic or torch.are_deterministic_algorithms_enabled():
             flags |= _lib.TRAIN_DETERMINISTIC
-        y = _NativeTrainStep.apply(self, flags, self._aligned(x), *params)
+        y = _NativeTrainStep.apply(self, flags, reducer, self._aligned(x), *params)
         if frozen_bn:
             return y                                         # running statistics untouched: the folded copies stay valid
         for blk in blocks:                                   # torch.nn.BatchNorm1d bookkeeping (momentum is not None: unused)
@@ -443,6 +490,29 @@ class Model(nn.Module):
         # the kernels updated running_mean / running_var through raw pointers (no _version bump): drop the folded copies
         self._native.invalidate_weights()
         return y
+
+    def _bn_sync_reducer(self):
+        """The cross-rank sum of a batch-statistics native step, or None for per-rank statistics. It syncs exactly when
+        ``nn.SyncBatchNorm`` would: every BatchNorm container is one (``nn.SyncBatchNorm.convert_sync_batchnorm(model)``),
+        ``torch.distributed`` is initialised and their process group (WORLD when None) has more than one rank. Some
+        containers converted and others not, or containers in different groups, raise ValueError. ``_bn_allreduce``, when
+        set, is the reducer regardless (tests, tools/sync_bn_bench.py)."""
+        if self._bn_allreduce is not None:
+            return self._bn_allreduce
+        bns = [blk[1] for blk in self._blocks()]
+        synced = [isinstance(bn, nn.SyncBatchNorm) for bn in bns]
+        if not any(synced):
+            return None
+        if not all(synced):
+            raise ValueError(f"{sum(synced)} of the {len(bns)} BatchNorm containers are nn.SyncBatchNorm: the native training "
+                             "step synchronises all of them or none (nn.SyncBatchNorm.convert_sync_batchnorm(model))")
+        if len({id(bn.process_group) for bn in bns}) > 1:
+            raise ValueError("the nn.SyncBatchNorm containers of this model use different process groups: the native "
+                             "training step synchronises all of them over one group")
+        group = bns[0].process_group
+        if not dist.is_available() or not dist.is_initialized() or dist.get_world_size(group) <= 1:
+            return None
+        return lambda buf: dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
 
     def _check_input(self, x: torch.Tensor):
         if x.dim() != 3 or x.size(1) != 1:
