@@ -94,6 +94,9 @@ size_t wunet_workspace_bytes(const wunet_ctx *ctx, int B, int T, int precision);
  * T must be a multiple of 2^n_layers (the reference raises from torch.cat at :95 otherwise)
  * -> WUNET_EINVAL.  Enqueues kernels on `stream` and returns; `workspace` must stay alive until
  * they finish.  Call sites this serves: trainer/trainer.py:75, enhancement.py:66.
+ * The tensor-core precisions (WUNET_PREC_BF16, _FP16, _FP32_TC) need channels_interval % 8 == 0 and <= 64; widths 40 .. 64 run
+ * without the forms gated on narrow channels (row-pair block 1, merged decoder tails, the group-of-8 block 0), with a block 0 whose
+ * tile shrinks with the width. WUNET_PREC_FP32 takes any channel plan.
  */
 int wunet_forward(wunet_ctx *ctx, const float *x_dev, float *y_dev, int B, int T, int precision,
                   void *workspace, size_t workspace_bytes, void *stream);
@@ -325,7 +328,8 @@ int wunet_debug_train_layout(int n_layers, int channels_interval, int B, int T, 
  *  [27] threads per CTA  [28] CTAs per SM  [29] grid  [30] small (two-CTAs-per-SM) flavour  [31] tiles per frame */
 int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity);
 /* The same query for a tensor-core precision: WUNET_PREC_BF16 (= wunet_debug_plan), WUNET_PREC_FP16 (the bf16 plan) or
- * WUNET_PREC_FP32_TC (the split-precision plan: no row-pair form, no dense GEMM, block 0 on CUDA cores). WUNET_PREC_FP32 -> WUNET_EINVAL. */
+ * WUNET_PREC_FP32_TC (the split-precision plan: no row-pair form, no dense GEMM, block 0 on CUDA cores). WUNET_PREC_FP32 -> WUNET_EINVAL.
+ * channels_interval up to 64 (a multiple of 8); [14] counts split-precision K-loop positions (three per 64-channel chunk). */
 int wunet_debug_plan_prec(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
                           int precision);
 

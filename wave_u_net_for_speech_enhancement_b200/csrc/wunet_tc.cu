@@ -93,7 +93,7 @@ struct TcLevel {
     const float *scale = nullptr, *shift = nullptr;
 };
 
-static int sp_chunk_order(const TcLevel &lv, bool dec, unsigned char *map, SplitTable *tab);
+static int sp_chunk_order(const TcLevel &lv, bool dec, unsigned char *map, SplitTable *tab, bool wide = false);
 
 struct TcPlanLevel {
     TcParams p;
@@ -292,8 +292,8 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
     st->out_w = out_w; st->out_b = out_b;
     st->plan_ws = nullptr;                               // weights moved: rebuild maps lazily
     st->f16_packed = false;                              // and repack fp16 on the next fp16 forward
-    derive_levels(st->levels, blocks, nblocks, n, st->merge);
-    if (ci % 8 != 0 || ci > 32) return 0;                // tensor-core path unsupported for this plan; forward reports it
+    derive_levels(st->levels, blocks, nblocks, n, st->merge && ci <= 32);     // no merged tail chunks in wide plans
+    if (ci % 8 != 0 || ci > 64) return 0;                // tensor-core path unsupported for this plan; forward reports it
     {
         // enc0 runs on CUDA cores from fp32 weights: keep a library-owned copy (include/wunet_b200.h: the caller's tensors are
         // only read during wunet_set_weights)
@@ -323,13 +323,19 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         }
         {
             // split-precision packing (fp32_tc): [K][Npad][positions * 64] in the split K-loop order
+            // (wide plans: more than 48 positions in the chunk form of wunet_tc_wide.cu)
             SplitTable tab;
-            lv.sp_chunks = sp_chunk_order(lv, i > n, nullptr, &tab);
+            lv.sp_chunks = sp_chunk_order(lv, i > n, nullptr, &tab, ci > 32);
             const size_t ns = (size_t)lv.k * lv.Npad * lv.sp_chunks * 64;
             if (!lv.wp_sp && cudaMalloc(&lv.wp_sp, ns * sizeof(__nv_bfloat16)) != cudaSuccess) return tc_fail("cudaMalloc(wp_sp) failed");
-            pack_tc_split_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(blocks[i].w, lv.wp_sp, lv.cout, lv.cin0 + lv.cin1, lv.k,
-                                                                                  lv.Npad, tab);
-            if (cudaGetLastError() != cudaSuccess) return tc_fail("pack_tc_split_kernel launch failed");
+            if (lv.sp_chunks > 48) {                        // (more than 3 x 48 positions, or a narrow plan: the planner refuses it)
+                if (ci > 32 && lv.sp_chunks <= 3 * 48 && wide::pack_split(blocks[i].w, lv.wp_sp, lv.cout, lv.cin0 + lv.cin1, lv.k, lv.Npad, tab, stream) != cudaSuccess)
+                    return tc_fail("pack_tc_split_wide_kernel launch failed");
+            } else {
+                pack_tc_split_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(blocks[i].w, lv.wp_sp, lv.cout, lv.cin0 + lv.cin1, lv.k,
+                                                                                      lv.Npad, tab);
+                if (cudaGetLastError() != cudaSuccess) return tc_fail("pack_tc_split_kernel launch failed");
+            }
         }
         if (lv.mg_s) {
             const size_t nm = (size_t)lv.k * lv.Npad * 64;
@@ -423,9 +429,11 @@ static int make_map(TcState *st, CUtensorMap *m, const void *base, uint64_t d0, 
 // upsampled chunks, skip chunks, partial upsampled chunk - or the partial one first if it is the only one): per chunk, hi
 // data x w_hi, the same operand stage x w_lo, lo data x w_hi. Fills chunk_map bytes (bit 7 upsampled segment, bit 6 low data part, bits 0-5 chunk
 // index) and the table the weight packing follows. Returns the number of positions.
-static int sp_chunk_order(const TcLevel &lv, bool dec, unsigned char *map, SplitTable *tab)
+// wide (channel plans wider than 32): a block of more than 48 positions gets the chunk form instead, which the SP = 2 kernels
+// read (chunk_info): map and table list the chunks, each standing for its three positions in the order above.
+static int sp_chunk_order(const TcLevel &lv, bool dec, unsigned char *map, SplitTable *tab, bool wide)
 {
-    unsigned char one[16];
+    unsigned char one[256];                 // chunks of the block: at most 2 n + 2
     int k = 0;
     const int n0 = (lv.cin0 + 63) / 64, n1 = (lv.cin1 + 63) / 64, nfull0 = lv.cin0 / 64;
     if (!dec) { for (int c = 0; c < n0; ++c) one[k++] = (unsigned char)c; }
@@ -436,6 +444,24 @@ static int sp_chunk_order(const TcLevel &lv, bool dec, unsigned char *map, Split
         for (int c = 0; c < nfull0; ++c) one[k++] = (unsigned char)(0x80 | c);
         for (int c = 0; c < n1; ++c) one[k++] = (unsigned char)c;
         if (nfull0 < n0) one[k++] = (unsigned char)(0x80 | nfull0);
+    }
+    if (3 * k > 48) {
+        // more positions than chunk_map holds: the chunk form (wide plans), or a count the planner refuses
+        if (wide && k <= 48) {
+            for (int c = 0; c < k; ++c) {
+                const bool up = dec && (one[c] & 0x80);
+                const int idx = one[c] & 0x1f;
+                if (map) map[c] = one[c];
+                if (tab) {
+                    const int seg = (up || !dec) ? lv.cin0 : lv.cin1;
+                    tab->base[c] = (short)(((up || !dec) ? 0 : lv.cin0) + 64 * idx);
+                    tab->width[c] = (unsigned char)std::min(64, seg - 64 * idx);
+                    tab->wlo[c] = 0;
+                }
+            }
+        }
+        if (tab) tab->n = 3 * k;
+        return k <= 48 ? 3 * k : 3 * 48 + 1;
     }
     int n = 0;
     auto put = [&](int c, bool lo_data, bool w_lo, bool reuse) {
@@ -464,8 +490,9 @@ static int sp_chunk_order(const TcLevel &lv, bool dec, unsigned char *map, Split
 // hd_mt > 0: the block is the last one and only the network output is wanted (head-only instantiation, see build_plan): M
 // sub-tiles per CTA for it, so that the ring of previous-level rows fits next to the input ring (small flavour only).
 // pair: row-pair mode - lv is the virtual block (doubled channel counts, pair taps) and the frames are half as long.
+// wide: the plan's channels_interval is above 32 (split precision may then take the chunk form, p.split = 2).
 static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms, const std::string &ovr, TcPlanLevel &P, bool sp = false,
-                      int hd_mt = 0, bool pair = false, bool group8 = false)
+                      int hd_mt = 0, bool pair = false, bool group8 = false, bool wide = false)
 {
     TcParams &p = P.p;
     memset(&p, 0, sizeof(p));
@@ -484,8 +511,8 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
         // upsampled chunk: a TMA chunk is never preceded by a short chunk, so its load latency hides behind MMAs.
         int k = 0;
         if (sp) {
-            p.split = 1;
-            p.nchunks = sp_chunk_order(lv, dec, p.chunk_map, nullptr);
+            p.nchunks = sp_chunk_order(lv, dec, p.chunk_map, nullptr, wide);
+            p.split = (wide && p.nchunks > 48) ? 2 : 1;  // 2: chunk_map lists chunks (SP = 2 kernels)
         } else if (!dec) { for (int c = 0; c < p.nchunks; ++c) p.chunk_map[k++] = (unsigned char)c; }
         else if (pair) {
             // row-pair decoder: all upsampled chunks first (they are produced in one phase into consecutive ring stages), then the skip chunks
@@ -517,7 +544,7 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
                 if (nfull0 < p.nchunks0) p.chunk_map[k++] = (unsigned char)(0x80 | nfull0);
             }
         }
-        if (p.nchunks > 48) return tc_fail("too many K chunks");
+        if (p.nchunks > (p.split == 2 ? 3 * 48 : 48)) return tc_fail("too many K chunks");
     }
     // ---- tiling ---------------------------------------------------------------------------------
     TcOverride ov = parse_override(ovr, i);
@@ -639,7 +666,7 @@ static int plan_block(const TcLevel &lv, int i, int n, int B, int T, int num_sms
     if (P.smem > (size_t)kSmemLimit) return tc_fail("level %d: smem %zu too large", i, P.smem);
 
     const bool last_block = (i == 2 * n);
-    if (last_block && lv.cout > (pair ? 64 : 32)) return tc_fail("fused head needs channels_interval <= 32");
+    if (last_block && lv.cout > 64) return tc_fail("fused head needs channels_interval <= 64");
     if (dec && pair && p.na < p.nchunks0) return tc_fail("level %d: the row-pair producers fill %d ring stages at once, the ring has %d", i, p.nchunks0, p.na);
     if (last_block && p.packed) return tc_fail("bf16 path needs frames of at least 128 samples (T=%d): the fused head works on full frames", T);
     if (last_block && p.nsplit != 1) return tc_fail("fused head needs the whole channel range in one CTA");
@@ -774,7 +801,7 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
                 return -1;
             continue;
         }
-        if (plan_block(lv, i, n, B, T, st->num_sms, st->plan_ovr, P, sp, 0, pair)) return -1;
+        if (plan_block(lv, i, n, B, T, st->num_sms, st->plan_ovr, P, sp, 0, pair, false, st->ci > 32)) return -1;
         TcParams &p = P.p;
         const bool dec = i > n;
         const int L = p.L;
@@ -835,7 +862,7 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
     const char *e0 = getenv("WUNET_TC_ENC0");
     const bool g8 = mode == 0 && block == 0 && e0 && e0[0] == '1';    // block 0 has a tensor-core plan only in its group-of-8 form (bf16)
     if (nblocks != 2 * n + 1 || (block < 1 && !g8) || block >= nblocks) return tc_fail("block %d out of range (1..%d)", block, 2 * n);
-    if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
+    if (ci % 8 != 0 || ci > 64) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 64 (got %d)", ci);
     if (cap < 32 || !f) return tc_fail("need room for 32 fields");
     if (g8) {
         if (blocks[0].k != 15 || blocks[0].cin != 1 || 8 * blocks[0].cout > 256 || T % 8 != 0 || T / 8 < 128) return tc_fail("block 0 has no group-of-8 plan for this shape");
@@ -854,7 +881,7 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
     }
     std::vector<TcLevel> levels(nblocks);
     const char *mge = getenv("WUNET_TC_MERGE");
-    derive_levels(levels, blocks, nblocks, n, !(mge && mge[0] == '0'));
+    derive_levels(levels, blocks, nblocks, n, !(mge && mge[0] == '0') && ci <= 32);
     const char *ovr = getenv("WUNET_TC_OVR");
     TcPlanLevel P{};
     const std::string ovr_s = ovr ? ovr : "";
@@ -862,7 +889,7 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
     bool planned = false;
     if (mode == 1) {
         // split precision (fp32_tc): every block on conv_tc_kernel in split form, no row-pair form, no dense GEMM (build_plan)
-        if (plan_block(levels[block], block, n, B, T, num_sms, ovr_s, P, true, 0)) return -1;
+        if (plan_block(levels[block], block, n, B, T, num_sms, ovr_s, P, true, 0, false, false, ci > 32)) return -1;
         planned = true;
     } else {
         // bf16 and fp16: row-pair mode of block 1 (WUNET_TC_PAIR bit 0), planned like build_plan does
@@ -928,7 +955,7 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
 {
     if (!st) return tc_fail("tensor-core state missing");
     const int ci = st->ci;
-    if (ci % 8 != 0 || ci > 32) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 32 (got %d)", ci);
+    if (ci % 8 != 0 || ci > 64) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 64 (got %d)", ci);
     if (!st->attr_set) {
         cudaFuncSetAttribute(conv_tc_kernel<15, false, kEpiWarpsLarge, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
         cudaFuncSetAttribute(conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
@@ -946,6 +973,7 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
         cudaFuncSetAttribute(enc0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         cudaFuncSetAttribute(enc0_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         f16::set_smem_attributes();
+        wide::set_smem_attributes();
         int dev = 0, sms = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
             st->dev_sms = sms;
@@ -1009,7 +1037,9 @@ static int launch_enc0(TcState *st, const float *x, int f0, int nf, int T, void 
         const int total = nf * ((T + 1023) / 1024);
         cfg.gridDim = dim3((unsigned)std::min(total, st->num_sms * 4), 1, 1);
     }
-    if (st->plan_mode == 2)                             // fp16: the same kernels with fp16 rows (same size as bf16 ones)
+    if (st->ci > 32)                                    // wide plans: a tile that shrinks with C (no even-row copy: no row-pair form)
+        wide::launch_enc0(cfg, st->plan_mode, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C);
+    else if (st->plan_mode == 2)                        // fp16: the same kernels with fp16 rows (same size as bf16 ones)
         f16::launch_enc0(cfg, persistent, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, even);
     else if (persistent)
         cudaLaunchKernelEx(&cfg, enc0_kernel_v2, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, split, even);
@@ -1059,6 +1089,9 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
         // row-pair mode of the first tensor-core encoder block: a 9-tap block over pairs of positions
         if (!P.small) cudaLaunchKernelEx(&cfg, conv_tc_kernel<9, false, kEpiWarpsLarge, 0, 0>, P.tmA, P.tmW, P.tmO, p);
         else cudaLaunchKernelEx(&cfg, conv_tc_kernel<9, false, kEpiWarpsSmall, 0, 0>, P.tmA, P.tmW, P.tmO, p);
+    } else if (p.split == 2) {
+        // split precision, more than 48 K-loop positions (wide plans): chunk_map lists chunks
+        cudaLaunchKernelEx(&cfg, wide::conv_split_kernel(P.upcat), P.tmA, P.tmW, P.tmO, p);
     } else if (p.split) {
         if (P.upcat) cudaLaunchKernelEx(&cfg, conv_tc_kernel<5, true, kEpiWarpsLarge, kProducerWarpsLarge, 0, 1>, P.tmA, P.tmW, P.tmO, p);
         else cudaLaunchKernelEx(&cfg, conv_tc_kernel<15, false, kEpiWarpsLarge, 0, 0, 1>, P.tmA, P.tmW, P.tmO, p);

@@ -211,4 +211,17 @@ cudaError_t expand_gemm_weights(const float *w, void *wx, size_t n, int Cout, in
 cudaError_t nlc_to_ncl(const void *src, float *dst, int B, int L, int C, cudaStream_t stream);
 }  // namespace f16
 
+// The kernels only wide channel plans (40 <= channels_interval <= 64) launch (wunet_tc_wide.cu).
+namespace wide {
+using ConvKernel = f16::ConvKernel;
+void set_smem_attributes();
+// block 0 with a tile that shrinks with C; mode 0 = bf16, 1 = split precision, 2 = fp16. Sets cfg's grid, block and shared memory.
+cudaError_t launch_enc0(cudaLaunchConfig_t cfg, int mode, const float *x, const float *w, const float *scale, const float *shift, void *out,
+                        int B, int T, int C);
+// split-precision conv form for blocks of more than 48 K-loop positions (chunk_map lists chunks: chunk_info, SP = 2); large flavour
+ConvKernel conv_split_kernel(bool upcat);
+// its weights: tab lists the chunks (base, width) and the positions (n = 3 x chunks)
+cudaError_t pack_split(const float *w, void *wp, int Cout, int Cin, int K, int Npad, const SplitTable &tab, cudaStream_t stream);
+}  // namespace wide
+
 }  // namespace wunet

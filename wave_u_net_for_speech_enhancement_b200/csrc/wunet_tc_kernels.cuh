@@ -140,12 +140,15 @@ __device__ __forceinline__ float tanh_fast(float x) { return 1.f - __fdividef(2.
 }  // namespace
 
 // K-loop position c -> (segment, chunk index inside the segment, K16 steps, 64-wide slot in the packed weights)
+// SP = 2 (split precision, wide channel plans, wunet_tc_wide.cu): chunk_map lists the 64-channel chunks, not the positions;
+// chunk q is positions 3q (hi data x w_hi), 3q + 1 (the same stage x w_lo) and 3q + 2 (lo data x w_hi), the order and flags
+// the SP = 1 map spells out per position. A block may then have up to 3 x 48 positions.
 struct ChunkInfo { bool up; int idx, nk, kslot; bool merged; int vo, nvec; bool lo, reuse; };
 template <bool UPCAT, int MG, int SP = 0>
 __device__ __forceinline__ ChunkInfo chunk_info(const TcParams &p, int c)
 {
     ChunkInfo ci;
-    const int m = p.chunk_map[c];
+    const int m = SP == 2 ? p.chunk_map[c / 3] | ((c % 3) == 1 ? 0x20 : 0) | ((c % 3) == 2 ? 0x40 : 0) : p.chunk_map[c];
     ci.lo = false; ci.reuse = false;
     if (SP != 0) {                                // split precision: the weight slot is the K-loop position itself
         ci.merged = false;
@@ -763,8 +766,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         if (SP != 0) {
                             // the chunk's lo-data position follows two positions later ([hi x w_hi, re-use x w_lo, lo x w_hi]): fill its
                             // stage (the next one of the ring) from the same interpolation instead of computing everything twice
-                            const bool pair = !cu.lo && c + 2 < p.nchunks && p.chunk_map[c + 2] == (p.chunk_map[c] | 0x40) &&
-                                              (p.chunk_map[c + 1] & 0x20);
+                            const bool pair = SP == 2 ? !cu.lo && c + 2 < p.nchunks
+                                                      : !cu.lo && c + 2 < p.nchunks && p.chunk_map[c + 2] == (p.chunk_map[c] | 0x40) &&
+                                                            (p.chunk_map[c + 1] & 0x20);
                             int sa2 = sa + 1, pa2 = pa;
                             if (sa2 == p.na) { sa2 = 0; pa2 ^= 1; }
                             if (pair) mbar_wait(a_empty + 8 * sa2, pa2 ^ 1);
@@ -951,6 +955,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
 }
 
+// WUNET_TC_CONV_ONLY (wunet_tc_wide.cu): the includer instantiates conv_tc_kernel forms of its own and needs none of the
+// non-template kernels below, which the other two units already emit.
+#ifndef WUNET_TC_CONV_ONLY
 // -------------------------------------------------------------------------------------------------
 // bottom of the U (frames of at most 16 samples): the block as ONE dense GEMM over frames
 // -------------------------------------------------------------------------------------------------
@@ -1450,3 +1457,5 @@ __global__ void nlc_f16_to_ncl_f32_kernel(const __half *__restrict__ src, float 
     const int b = (int)(i / ((long long)L * C));
     dst[i] = TcElem::to_f32(src[((size_t)b * L + l) * C + c]);
 }
+
+#endif  // WUNET_TC_CONV_ONLY

@@ -262,7 +262,7 @@ class Model(nn.Module):
     Extra keyword arguments (not in the reference; configs pass ``"args": {}`` so defaults apply):
 
     precision      "fp32_tc" (default): fp32-grade results on the tensor cores (bf16 hi + lo split, three MMAs per
-                   product; <=1e-4 vs the reference, measured 1e-6; needs channels_interval % 8 == 0 and <= 32);
+                   product; <=1e-4 vs the reference, measured 1e-6; needs channels_interval % 8 == 0 and <= 64);
                    "fp32": the same contract on CUDA-core FFMA for any channel plan (slower);
                    "bf16": bf16 activations / operands on the tensor cores (the fastest path; ~6e-4 on the output);
                    "fp16": the bf16 contract with fp16 activations / operands (11-bit significand, the precision of the
