@@ -1,7 +1,8 @@
-"""Model(train_precision=...) without a GPU: the constructor surface, and the bf16 training kernels of wunet_train_tc.cu compiled
-for sm_90a with ptxas in verbose mode (into a temporary directory, the in-tree library is untouched). ptxas must report both
-kernels and must not serialise their wgmma (C7520) or guard the accumulators with extra warpgroup arrives (C7519), as
-test_wgmma_issue_cpu.py checks for wunet_tc.cu."""
+"""Model(train_precision=...) without a GPU: the constructor surface, and the training tensor-core kernels of wunet_train_tc.cu
+(bf16 and tf32) compiled for sm_90a with ptxas in verbose mode (into a temporary directory, the in-tree library is untouched).
+ptxas must report the conv and weight-gradient kernels and must not serialise their wgmma (C7520) or guard the accumulators
+with extra warpgroup arrives (C7519), as test_wgmma_issue_cpu.py checks for wunet_tc.cu; test_train_tc_unit_cpu.py checks
+the unit kernel by kernel."""
 import copy
 import json
 import os
@@ -31,6 +32,10 @@ def test_train_tc_kernels_compile_without_wgmma_serialisation(tmp_path):
     log = r.stdout + r.stderr
     assert r.returncode == 0, log[-4000:]
     assert "train_conv_tc_kernel" in log and "train_wgrad_tc_kernel" in log
+    # the unit holds both precisions: per precision 16 convolutions, 6 weight gradients and 1 pack kernel
+    entries = re.findall(r"Compiling entry function '(\w+)'", log)
+    assert len(entries) == 46 and len([e for e in entries if "Tf32" in e or "tf32" in e]) == 23, entries
+    assert "train_wgrad_tf32_kernel" in log
     bad = [line for line in log.splitlines() if re.search(r"C75(19|20)", line)]
     assert not bad, "\n".join(bad[:10])
     assert not re.search(r"[1-9]\d* bytes spill stores", log), "spills in the training tensor-core kernels"

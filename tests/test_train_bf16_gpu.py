@@ -1,5 +1,5 @@
-"""Mixed-precision training step, Model(train_precision="bf16") (DESIGN §5.4): the bf16 tensor-core kernels of
-wunet_train_tc.cu pass by pass, the whole step against the float64 golden steps next to PyTorch's own autocast step, and a
+"""Mixed-precision training step, Model(train_precision="bf16") (DESIGN §5.4): the tensor-core kernels of wunet_train_tc.cu
+at bf16 pass by pass, the whole step against the float64 golden steps next to PyTorch's own autocast step, and a
 30-step Adam trajectory against the fp32 native step."""
 import os
 

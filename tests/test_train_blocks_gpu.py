@@ -1,5 +1,5 @@
-"""Teacher-forced check of every kernel of the native training step (csrc/wunet_train.cu, csrc/wunet_train_tc.cu,
-csrc/wunet_train_tf32.cu), block by block, against float64.
+"""Teacher-forced check of every kernel of the native training step (csrc/wunet_train.cu; csrc/wunet_train_tc.cu at bf16 and
+tf32), block by block, against float64.
 
 The step runs through wunet_train_forward_ex / wunet_train_backward_ex on a workspace this test allocates; every block's
 tensors are read as views given by the host-only layout query (wunet_debug_train_layout). For each block, what its kernels

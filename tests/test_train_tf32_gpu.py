@@ -1,4 +1,4 @@
-"""TF32 training step, Model(train_precision="tf32") (DESIGN §5.4): the tf32 tensor-core kernels of wunet_train_tf32.cu pass by
+"""TF32 training step, Model(train_precision="tf32") (DESIGN §5.4): the tensor-core kernels of wunet_train_tc.cu at tf32 pass by
 pass against float64, the whole step and the autograd goldens next to PyTorch's own fp32 step with cuDNN's TF32 convolutions
 (torch.backends.cudnn.allow_tf32, the reference's arithmetic on an H100), deterministic mode, and a 30-step Adam trajectory
 against the fp32 native step."""

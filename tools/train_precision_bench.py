@@ -2,7 +2,7 @@
 
     native fp32   Model(train_backend="native", train_precision="fp32")   fp32 FFMA convolutions (wunet_train.cu)
     native bf16   Model(train_backend="native", train_precision="bf16")   bf16 wgmma convolutions (wunet_train_tc.cu)
-    native tf32   Model(train_backend="native", train_precision="tf32")   tf32 wgmma convolutions (wunet_train_tf32.cu)
+    native tf32   Model(train_backend="native", train_precision="tf32")   tf32 wgmma convolutions (wunet_train_tc.cu)
     *_det         the same three under torch.backends.cudnn.deterministic = True: deterministic mode (ordered weight- and
                   head-gradient sums instead of float atomics)
     autocast      Model(train_backend="torch") under torch.autocast("cuda", torch.bfloat16): PyTorch eager + cuDNN

@@ -74,30 +74,23 @@ int launch_pack_fp32(const float *w, const float *bias, const float *g, const fl
                      const float *var, float *wp, float *scale, float *shift, int Cout, int Cin, int K,
                      cudaStream_t st);
 
-// ---- bf16 tensor-core training convolutions, implemented in wunet_train_tc.cu -----------------------
-// launch_conv_bf16: launch_conv_fp32's operator with a.wp pointing at the bf16 forward (or input-gradient) packing written by
-// train_tc_pack; ksize 15 (DIRECT, DECIM) or 5 (DIRECT, UPCAT).
-int launch_conv_bf16(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
+// ---- tensor-core training convolutions, implemented in wunet_train_tc.cu ------------------------------------------------
+// prec (TrainPrec, wunet_train.cuh) is TRAIN_BF16 (bf16 operands, round to nearest) or TRAIN_TF32 (tf32 operands, round to
+// nearest, ties away: cvt.rna.tf32.f32); products are accumulated in fp32.
+// launch_train_conv_tc: launch_conv_fp32's operator with a.wp pointing at the forward (or input-gradient) packing written by
+// train_tc_pack at the same precision; ksize 15 (DIRECT, DECIM) or 5 (DIRECT, UPCAT).
+int launch_train_conv_tc(int prec, const ConvArgs &a, int ksize, int mode, cudaStream_t st);
 // dw[co][ci][k] += sum_{b,l} dz[b][co][l] * in(b, ci, l + k - pad), in read through `a` as the forward reads it (dw zeroed first).
 // slices = true: slice z of the grid stores its partial sums to dw + z * Cout * Cin * K instead (nothing zeroed first)
-int launch_wgrad_bf16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices = false);
-// Launch geometry of the two weight-gradient kernels, the one definition their launchers and wunet_debug_train_layout use:
+int launch_train_wgrad_tc(int prec, const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st,
+                          bool slices = false);
+// Launch geometry of the weight-gradient kernels, the one definition their launchers and wunet_debug_train_layout use:
 // grid, number of (frame, position tile) work items that gridDim.z slices share, and positions per item.
 struct WgradGrid { dim3 grid; int items, positions; };
 WgradGrid wgrad_grid_fp32(int B, int L, int Cin, int Cout);             // train_wgrad_kernel (wunet_train.cu)
-WgradGrid wgrad_grid_bf16(int B, int L, int Cin, int Cout, int ksize);  // train_wgrad_tc_kernel (wunet_train_tc.cu)
-// bf16 elements of one packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout))
-size_t train_tc_packed_elems(int cout, int cin, int k);
-int train_tc_pack(const float *w, __nv_bfloat16 *wf, __nv_bfloat16 *wb, int Cout, int Cin, int K, cudaStream_t st);
-
-// ---- tf32 tensor-core training convolutions, implemented in wunet_train_tf32.cu ------------------------------
-// The same three operators as the bf16 launchers above, with tf32 operands (round to nearest, ties away: cvt.rna.tf32.f32);
-// a.wp points at the tf32 packing written by train_tf32_pack.
-int launch_conv_tf32(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
-int launch_wgrad_tf32(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices = false);
-WgradGrid wgrad_grid_tf32(int B, int L, int Cin, int Cout, int ksize);  // train_wgrad_tf32_kernel
-// fp32 elements of one tf32 packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout))
-size_t train_tf32_packed_elems(int cout, int cin, int k);
-int train_tf32_pack(const float *w, float *wf, float *wb, int Cout, int Cin, int K, cudaStream_t st);
+WgradGrid wgrad_grid_tc(int B, int L, int Cin, int Cout, int ksize);    // the tensor-core ones, at both precisions
+// bytes of one packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout)); a multiple of 256
+size_t train_tc_packed_bytes(int prec, int cout, int cin, int k);
+int train_tc_pack(int prec, const float *w, void *wf, void *wb, int Cout, int Cin, int K, cudaStream_t st);
 
 }  // namespace wunet

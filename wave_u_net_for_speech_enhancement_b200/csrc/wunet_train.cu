@@ -10,9 +10,9 @@
 // scratch region after the workspace layout and summed in an order fixed by the shapes (train_slice_sum_kernel,
 // train_head_sum_kernel); every other reduction of the step already has a fixed order.
 // The naive one-thread-per-output kernels they replace are kept as WUNET_TRAIN_NAIVE=1 (cross-check, tests).
-// TRAIN_BF16 (Model(train_precision="bf16")): the forward conv, input gradient and weight gradient of every block but the
-// first (Cin = 1) run on the bf16 tensor-core kernels of wunet_train_tc.cu instead; everything else is the same fp32 code.
-// TRAIN_TF32 (Model(train_precision="tf32")): likewise on the tf32 tensor-core kernels of wunet_train_tf32.cu.
+// TRAIN_BF16 / TRAIN_TF32 (Model(train_precision="bf16" / "tf32")): the forward conv, input gradient and weight gradient of
+// every block but the first (Cin = 1) run on the tensor-core kernels of wunet_train_tc.cu at that operand precision instead;
+// everything else is the same fp32 code.
 // TRAIN_FROZEN_BN (eval-mode BatchNorm: running statistics, never updated) and TRAIN_NO_PARAM_GRADS (input gradient only) only
 // change the BatchNorm arithmetic and which reductions run; the convolution-shaped passes are the same kernels. The input
 // gradient dx is train_input_grad_kernel below (head's raw-input channel + block 0's transposed conv).
@@ -696,8 +696,8 @@ struct Layout {
     std::vector<size_t> z, act, ga;      // float offsets of the pre-BN outputs, activations, activation gradients
     std::vector<size_t> mean, invstd, s1, s2;
     std::vector<size_t> wf, wb;          // the step's packed weights: forward / input-gradient operand layouts
-    std::vector<size_t> wf16, wb16;      // TRAIN_BF16 only (appended after `total` of the fp32 layout): the bf16 packings
-    std::vector<size_t> wftf, wbtf;      // TRAIN_TF32 only (appended likewise): the tf32 packings
+    std::vector<size_t> wftc, wbtc;      // TRAIN_BF16 / TRAIN_TF32 only (appended after `total` of the fp32 layout): the
+                                         // tensor-core packings at that precision
     size_t din, ones, zeros, total;      // ones / zeros: [kMaxC] identity scale and zero shift for the linear conv epilogue
 };
 constexpr int kMaxC = 2048;
@@ -708,18 +708,7 @@ bool on_tc(int prec, int i) { return (prec == TRAIN_BF16 || prec == TRAIN_TF32) 
 // launch geometry of block i's weight gradient at `prec`
 WgradGrid wgrad_grid_of(int prec, int i, int B, int L, int cin, int cout, int k)
 {
-    if (!on_tc(prec, i)) return wgrad_grid_fp32(B, L, cin, cout);
-    return prec == TRAIN_TF32 ? wgrad_grid_tf32(B, L, cin, cout, k) : wgrad_grid_bf16(B, L, cin, cout, k);
-}
-
-// the tensor-core launchers of `prec` (TRAIN_BF16 or TRAIN_TF32)
-int launch_conv_tc_prec(int prec, const ConvArgs &a, int ksize, int mode, cudaStream_t st)
-{
-    return prec == TRAIN_TF32 ? launch_conv_tf32(a, ksize, mode, st) : launch_conv_bf16(a, ksize, mode, st);
-}
-int launch_wgrad_tc_prec(int prec, const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices)
-{
-    return prec == TRAIN_TF32 ? launch_wgrad_tf32(a, dz, dw, ksize, mode, st, slices) : launch_wgrad_bf16(a, dz, dw, ksize, mode, st, slices);
+    return on_tc(prec, i) ? wgrad_grid_tc(B, L, cin, cout, k) : wgrad_grid_fp32(B, L, cin, cout);
 }
 
 void layout_of(const std::vector<Shape> &sh, int B, Layout &lo, int prec = TRAIN_FP32)
@@ -737,16 +726,11 @@ void layout_of(const std::vector<Shape> &sh, int B, Layout &lo, int prec = TRAIN
     }
     lo.din = take(din_max);
     lo.ones = take(kMaxC); lo.zeros = take(kMaxC);
-    lo.wf16.assign(nb, 0); lo.wb16.assign(nb, 0); lo.wftf.assign(nb, 0); lo.wbtf.assign(nb, 0);
+    lo.wftc.assign(nb, 0); lo.wbtc.assign(nb, 0);
     for (size_t i = 0; i < nb; ++i) {
         if (!on_tc(prec, (int)i)) continue;
-        if (prec == TRAIN_TF32) {
-            lo.wftf[i] = take(train_tf32_packed_elems(sh[i].cout, sh[i].cin, sh[i].k));
-            lo.wbtf[i] = take(train_tf32_packed_elems(sh[i].cin, sh[i].cout, sh[i].k));
-            continue;
-        }
-        lo.wf16[i] = take((train_tc_packed_elems(sh[i].cout, sh[i].cin, sh[i].k) + 1) / 2);        // float units
-        lo.wb16[i] = take((train_tc_packed_elems(sh[i].cin, sh[i].cout, sh[i].k) + 1) / 2);
+        lo.wftc[i] = take((train_tc_packed_bytes(prec, sh[i].cout, sh[i].cin, sh[i].k) + 3) / 4);       // float units
+        lo.wbtc[i] = take((train_tc_packed_bytes(prec, sh[i].cin, sh[i].cout, sh[i].k) + 3) / 4);
     }
     lo.total = cur;
 }
@@ -821,7 +805,7 @@ int train_debug_layout(int n, int ci, int B, int T, int prec, int block, long lo
         (long long)lo.z[block] * b, (long long)lo.act[block] * b, (long long)lo.ga[block] * b, (long long)lo.mean[block] * b,
         (long long)lo.invstd[block] * b, (long long)lo.s1[block] * b, (long long)lo.s2[block] * b,
         s.cin, s.cin0, s.cin1, s.cout, s.L, s.k, s.mode,
-        tc ? (prec == TRAIN_TF32 ? 2 : 1) : 0, g.grid.x, g.grid.y, gz, g.items, g.positions, (g.items + gz - 1) / gz, (long long)lo.total * b};
+        tc ? prec : 0 /* the field's 1 = bf16, 2 = tf32 are TRAIN_BF16, TRAIN_TF32 */, g.grid.x, g.grid.y, gz, g.items, g.positions, (g.items + gz - 1) / gz, (long long)lo.total * b};
     for (int i = 0; i < kTrainLayoutFields; ++i) f[i] = v[i];
     return 0;
 }
@@ -858,17 +842,11 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
         ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
         float *z = ws + lo.z[i];
         const dim3 grid((unsigned)((s.L + 127) / 128), (unsigned)((s.cout + 7) / 8), (unsigned)B);
-        if (on_tc(prec, i) && prec == TRAIN_TF32) {
-            // z = conv(tf32(in), tf32(w)) + bias on the tensor cores (fp32 accumulate); both tf32 packings for this step
-            if (train_tf32_pack(P.conv_w[i], ws + lo.wftf[i], ws + lo.wbtf[i], s.cout, s.cin, s.k, st) < 0) return train_fail("training forward, block %d: tf32 pack failed", i);
-            a.wp = ws + lo.wftf[i]; a.scale = ws + lo.ones; a.shift = P.conv_b[i]; a.out = z; a.linear = 1;
-            if (launch_conv_tf32(a, s.k, s.mode, st) < 0) return train_fail("training forward, block %d: tf32 conv launch failed", i);
-        } else if (on_tc(prec, i)) {
-            // z = conv(bf16(in), bf16(w)) + bias on the tensor cores (fp32 accumulate); both bf16 packings for this step
-            __nv_bfloat16 *wf16 = reinterpret_cast<__nv_bfloat16 *>(ws + lo.wf16[i]), *wb16 = reinterpret_cast<__nv_bfloat16 *>(ws + lo.wb16[i]);
-            if (train_tc_pack(P.conv_w[i], wf16, wb16, s.cout, s.cin, s.k, st) < 0) return train_fail("training forward, block %d: bf16 pack failed", i);
-            a.wp = reinterpret_cast<const float *>(wf16); a.scale = ws + lo.ones; a.shift = P.conv_b[i]; a.out = z; a.linear = 1;
-            if (launch_conv_bf16(a, s.k, s.mode, st) < 0) return train_fail("training forward, block %d: bf16 conv launch failed", i);
+        if (on_tc(prec, i)) {
+            // z = conv(round(in), round(w)) + bias on the tensor cores (fp32 accumulate); both packings for this step
+            if (train_tc_pack(prec, P.conv_w[i], ws + lo.wftc[i], ws + lo.wbtc[i], s.cout, s.cin, s.k, st) < 0) return train_fail("training forward, block %d: tensor-core pack failed", i);
+            a.wp = ws + lo.wftc[i]; a.scale = ws + lo.ones; a.shift = P.conv_b[i]; a.out = z; a.linear = 1;
+            if (launch_train_conv_tc(prec, a, s.k, s.mode, st) < 0) return train_fail("training forward, block %d: tensor-core conv launch failed", i);
         } else if (!naive) {
             // z = conv(in, w) + bias through the tuned fp32 conv kernels: identity scale, shift = conv bias, no activation
             const long long nw = (long long)s.cout * s.cin * s.k;
@@ -971,7 +949,7 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
             if (!det) cudaMemsetAsync(G.conv_w[i], 0, (size_t)nw * sizeof(float), st);
             const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
             if (on_tc(prec, i)) {
-                if (launch_wgrad_tc_prec(prec, a, ga, wdst, s.k, s.mode, st, det) < 0) return train_fail("training backward, block %d: tensor-core weight-gradient launch failed", i);
+                if (launch_train_wgrad_tc(prec, a, ga, wdst, s.k, s.mode, st, det) < 0) return train_fail("training backward, block %d: tensor-core weight-gradient launch failed", i);
             } else if (!naive) {
                 launch_wgrad_fp32(a, ga, wdst, s.mode, st, det);
             } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
@@ -992,8 +970,8 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
                 d.src0 = ga; d.wp = ws + lo.wb[i]; d.scale = ws + lo.ones; d.shift = ws + lo.zeros; d.out = din;
                 d.B = B; d.L = s.L; d.Cin = s.cout; d.Cin0 = s.cout; d.Cin1 = 0; d.Cout = s.cin; d.linear = 1;
                 if (on_tc(prec, i)) {
-                    d.wp = ws + (prec == TRAIN_TF32 ? lo.wbtf[i] : lo.wb16[i]);      // the packing the forward wrote
-                    if (launch_conv_tc_prec(prec, d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: tensor-core input-gradient launch failed", i);
+                    d.wp = ws + lo.wbtc[i];                                     // the packing the forward wrote
+                    if (launch_train_conv_tc(prec, d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: tensor-core input-gradient launch failed", i);
                 } else if (launch_conv_fp32(d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: input-gradient conv launch failed", i);
             } else if (s.k == 15) train_conv_bwd_data_kernel<15><<<gd, 128, 0, st>>>(ga, P.conv_w[i], din, B, s.cin, s.cout, s.L);
             else train_conv_bwd_data_kernel<5><<<gd, 128, 0, st>>>(ga, P.conv_w[i], din, B, s.cin, s.cout, s.L);
@@ -1035,37 +1013,31 @@ int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int 
     a.up_scale = (mode == SRC_UPCAT && L > 1) ? (float)(L / 2 - 1) / (float)(L - 1) : 0.f;
     float *buf = nullptr;
     const size_t nw = (size_t)Cout * Cin * K, cpad = (cmax + 63) / 64 * 64, wpad = (nw + 63) / 64 * 64;      // 256-byte aligned parts
-    const size_t n16 = train_tc_packed_elems(Cout, Cin, K) + train_tc_packed_elems(Cin, Cout, K);
-    const size_t ntf = train_tf32_packed_elems(Cout, Cin, K) + train_tf32_packed_elems(Cin, Cout, K);
-    const size_t ntc = prec == TRAIN_TF32 ? ntf : (n16 + 1) / 2;                                  // float units
+    const bool tc = prec != TRAIN_FP32;
+    const size_t ntcf = tc ? train_tc_packed_bytes(prec, Cout, Cin, K) / sizeof(float) : 0;     // float units
+    const size_t ntc = tc ? ntcf + train_tc_packed_bytes(prec, Cin, Cout, K) / sizeof(float) : 0;
     if (cudaMalloc(&buf, (2 * cpad + 2 * wpad + ntc) * sizeof(float)) != cudaSuccess)
         return train_fail("debug conv: %s", cudaGetErrorString(cudaGetLastError()));
-    float *ones = buf, *zeros = buf + cpad, *wf = zeros + cpad, *wb = wf + wpad;
-    __nv_bfloat16 *wf16 = reinterpret_cast<__nv_bfloat16 *>(wb + wpad), *wb16 = wf16 + train_tc_packed_elems(Cout, Cin, K);
-    float *wftf = wb + wpad, *wbtf = wftf + train_tf32_packed_elems(Cout, Cin, K);
+    float *ones = buf, *zeros = buf + cpad, *wf = zeros + cpad, *wb = wf + wpad, *wtc_f = wb + wpad, *wtc_b = wtc_f + ntcf;
     const cudaStream_t st = 0;
     train_fill_kernel<<<(cmax + 255) / 256, 256, 0, st>>>(ones, 1.f, cmax);
     train_fill_kernel<<<(cmax + 255) / 256, 256, 0, st>>>(zeros, 0.f, cmax);
-    const bool tc = prec != TRAIN_FP32;
-    const float *wtc_f = prec == TRAIN_TF32 ? wftf : reinterpret_cast<const float *>(wf16);
-    const float *wtc_b = prec == TRAIN_TF32 ? wbtf : reinterpret_cast<const float *>(wb16);
     int rc = 0;
     if (pass == 2) {
         cudaMemsetAsync(out, 0, nw * sizeof(float), st);
-        if (tc) rc = launch_wgrad_tc_prec(prec, a, dz, out, K, mode, st, false);
+        if (tc) rc = launch_train_wgrad_tc(prec, a, dz, out, K, mode, st, false);
         else launch_wgrad_fp32(a, dz, out, mode, st);
     } else {
-        if (prec == TRAIN_TF32) rc = train_tf32_pack(w, wftf, wbtf, Cout, Cin, K, st);
-        else if (tc) rc = train_tc_pack(w, wf16, wb16, Cout, Cin, K, st);
+        if (tc) rc = train_tc_pack(prec, w, wtc_f, wtc_b, Cout, Cin, K, st);
         else train_pack_kernel<<<blocks_for((long long)nw, 256), 256, 0, st>>>(w, wf, wb, Cout, Cin, K);
         if (pass == 0) {
             a.wp = tc ? wtc_f : wf; a.scale = ones; a.shift = zeros; a.out = out; a.linear = 1;
-            if (rc >= 0) rc = tc ? launch_conv_tc_prec(prec, a, K, mode, st) : launch_conv_fp32(a, K, mode, st);
+            if (rc >= 0) rc = tc ? launch_train_conv_tc(prec, a, K, mode, st) : launch_conv_fp32(a, K, mode, st);
         } else {
             ConvArgs d{};
             d.src0 = dz; d.wp = tc ? wtc_b : wb; d.scale = ones; d.shift = zeros; d.out = out;
             d.B = B; d.L = L; d.Cin = Cout; d.Cin0 = Cout; d.Cin1 = 0; d.Cout = Cin; d.linear = 1;
-            if (rc >= 0) rc = tc ? launch_conv_tc_prec(prec, d, K, SRC_DIRECT, st) : launch_conv_fp32(d, K, SRC_DIRECT, st);
+            if (rc >= 0) rc = tc ? launch_train_conv_tc(prec, d, K, SRC_DIRECT, st) : launch_conv_fp32(d, K, SRC_DIRECT, st);
         }
     }
     const cudaError_t e = cudaDeviceSynchronize();

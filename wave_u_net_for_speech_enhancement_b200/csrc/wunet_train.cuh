@@ -25,7 +25,8 @@ struct TrainGrads {
 // Arithmetic of the three convolution-shaped passes. TRAIN_FP32: fp32 FFMA. TRAIN_BF16: bf16 operands (block input, weights,
 // dz; round to nearest), fp32 accumulation on the tensor cores (wunet_train_tc.cu); the first block stays fp32. Everything else
 // is fp32 at every precision. The workspace of TRAIN_BF16 is the fp32 one plus the bf16 weight packings. TRAIN_TF32: the same
-// with tf32 operands (round to nearest, ties away; wunet_train_tf32.cu), its workspace the fp32 one plus the tf32 packings.
+// with tf32 operands (round to nearest, ties away; the same kernels, templated on the operand type), its workspace the fp32
+// one plus the tf32 packings.
 enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1, TRAIN_TF32 = 2 };
 // TRAIN_FROZEN_BN: BatchNorm normalises by the running statistics and never updates them (eval-mode BatchNorm); the forward
 // and the backward of one step must agree on it. TRAIN_NO_PARAM_GRADS (backward only): no parameter gradient is computed

@@ -1,5 +1,5 @@
 // wunet_wgmma.cuh — sm_90a device helpers shared by the tensor-core kernels (wunet_tc.cu, wunet_tc_f16.cu: inference forward;
-// wunet_train_tc.cu: bf16 training convolutions; wunet_train_tf32.cu: tf32 training convolutions). Raw PTX; forms taken
+// wunet_train_tc.cu: bf16 and tf32 training convolutions). Raw PTX; forms taken
 // from the PTX ISA as shipped in CUDA 12.9.
 #pragma once
 #include <cuda_runtime.h>
