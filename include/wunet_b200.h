@@ -265,6 +265,34 @@ int wunet_train_backward_ex(wunet_ctx *ctx, const float *x, const float *y, cons
                             const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
                             float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                             void *stream, float *dx, int part, int precision, int flags);
+/* The same step with per-block BatchNorm modes and momenta and per-parameter gradients: fine-tuning with frozen layers
+ * (model.train() with some BatchNorm containers in .eval(), some parameters with requires_grad False).
+ * wunet_train_forward_blocks: the arguments of wunet_train_forward_ex, plus
+ *   bn_frozen[2n+1] (NULL = none): nonzero = that block's BatchNorm normalises by, and keeps, its running statistics (an
+ *     eval-mode container); WUNET_TRAIN_FROZEN_BN in flags freezes every block whatever bn_frozen says;
+ *   momenta[2n+1] (NULL = `momentum` for every block): each block's running-statistics factor (ignored for frozen blocks).
+ *   The one-value-per-channel check applies only when the middle block has batch statistics; the all-reduce hook (if
+ *   installed) is called only for blocks with batch statistics. With both arrays NULL this is wunet_train_forward_ex.
+ * wunet_train_backward_blocks: the arguments of wunet_train_backward_ex, plus bn_frozen, which must equal the forward's.
+ *   A NULL array among g_conv_w, g_conv_b, g_bn_weight, g_bn_bias, or a NULL entry in one, or a NULL g_out_w / g_out_b,
+ *   is a frozen parameter: nothing is computed for it and nothing is written. WUNET_TRAIN_NO_PARAM_GRADS freezes all of them.
+ *   Per block, the BatchNorm reduction runs when the block has batch statistics or its weight or bias gets a gradient, the
+ *   bias sum when g_conv_b[i] is set and the weight-gradient pass when g_conv_w[i] is set, each with the kernels, grids and
+ *   summation order of the full step (bit for bit the same values, deterministic mode included). Early stop: below the
+ *   lowest block that gets a gradient (block 0 when dx is requested) nothing is issued, and that block skips its input
+ *   gradient; a part with nothing to do returns at once. In a split backward that requests dx, pass dx to part 0 as well:
+ *   part 0 writes nothing there but keeps the gradient flowing to the middle block for part 1. Same workspace as the _ex
+ *   pair. */
+int wunet_train_forward_blocks(wunet_ctx *ctx, const float *x, float *y, int B, int T, const float *const *conv_w,
+                               const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                               float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                               float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags,
+                               const unsigned char *bn_frozen, const float *momenta);
+int wunet_train_backward_blocks(wunet_ctx *ctx, const float *x, const float *y, const float *dy, int B, int T,
+                                const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                                const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                                float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                                void *stream, float *dx, int part, int precision, int flags, const unsigned char *bn_frozen);
 /* BatchNorm statistics synchronised over data-parallel ranks: what nn.SyncBatchNorm (torch.nn.SyncBatchNorm.
  * convert_sync_batchnorm(model)) computes in a one-process-per-GPU step. With a hook installed, every training forward with
  * batch statistics (not WUNET_TRAIN_FROZEN_BN) on this context, and its backward, compute the BatchNorm reductions from sums

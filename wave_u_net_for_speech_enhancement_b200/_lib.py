@@ -81,6 +81,8 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_backward_part_prec.argtypes = lib.wunet_train_backward_part.argtypes + [ci]
     lib.wunet_train_forward_ex.argtypes = lib.wunet_train_forward_prec.argtypes + [ci]
     lib.wunet_train_backward_ex.argtypes = lib.wunet_train_backward.argtypes + [vp, ci, ci, ci]
+    lib.wunet_train_forward_blocks.argtypes = lib.wunet_train_forward_ex.argtypes + [vp, vp]
+    lib.wunet_train_backward_blocks.argtypes = lib.wunet_train_backward_ex.argtypes + [vp]
     lib.wunet_train_set_bn_allreduce.argtypes = [vp, BN_ALLREDUCE_FN, vp, vp, cs]
     lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     lib.wunet_debug_train_layout.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ll), ci]
@@ -101,7 +103,7 @@ EXPORTED_SYMBOLS = [
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
     "wunet_train_forward_ex", "wunet_train_backward_ex", "wunet_train_workspace_bytes_ex", "wunet_debug_train_layout",
-    "wunet_train_set_bn_allreduce",
+    "wunet_train_set_bn_allreduce", "wunet_train_forward_blocks", "wunet_train_backward_blocks",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]

@@ -528,21 +528,31 @@ int wunet_train_forward_prec(wunet_ctx *c, const float *x, float *y, int B, int 
                                   out_b, momentum, workspace, workspace_bytes, stream, precision, 0);
 }
 
-int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
-                           const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
-                           float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
-                           float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags)
+// wunet_train_forward_ex and wunet_train_forward_blocks: bn_frozen / momenta null = every block as `flags` and `momentum` say
+static int train_forward_impl(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
+                              const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                              float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                              float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags,
+                              const unsigned char *bn_frozen, const float *momenta)
 {
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
     const int prec = train_prec(precision);
     if (prec < 0) return WUNET_EINVAL;
     if (flags & ~kTrainFlags) return fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
+    const int nb = 2 * c->n + 1;
+    const bool all_frozen = flags & WUNET_TRAIN_FROZEN_BN;
+    bool any_batch = !all_frozen;
+    if (bn_frozen && !all_frozen) {
+        any_batch = false;
+        for (int i = 0; i < nb; ++i) any_batch = any_batch || !bn_frozen[i];
+    }
     // batch statistics of one value per channel (B = 1 and L = 1 at the middle block): torch.nn.BatchNorm1d raises in training
     // mode rather than normalise by a variance of 0. Synchronised statistics count every rank's frames (nn.SyncBatchNorm
     // raises only without other ranks).
-    const bool synced = c->bn_sync.fn && !(flags & WUNET_TRAIN_FROZEN_BN);
-    if (!(flags & WUNET_TRAIN_FROZEN_BN) && !synced && B == 1 && (T >> c->n) == 1)
+    const bool synced = c->bn_sync.fn && any_batch;
+    const bool middle_batch = !all_frozen && !(bn_frozen && bn_frozen[c->n]);
+    if (middle_batch && !synced && B == 1 && (T >> c->n) == 1)
         return fail(WUNET_EINVAL, "Expected more than 1 value per channel when training (B=1, T=%d: one value per channel at the "
                                   "middle block)", T);
     if (!x || !y || !workspace || !conv_w || !conv_b || !bn_weight || !bn_bias || !bn_running_mean || !bn_running_var || !out_w || !out_b)
@@ -552,10 +562,31 @@ int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T,
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "training workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b};
-    if (train_forward(c->n, c->ci, x, y, B, T, P, momentum, workspace, static_cast<cudaStream_t>(stream), prec, tflags,
-                      synced ? &c->bn_sync : nullptr))
+    std::vector<float> m(nb, momentum);
+    if (momenta) m.assign(momenta, momenta + nb);
+    if (train_forward(c->n, c->ci, x, y, B, T, P, m.data(), workspace, static_cast<cudaStream_t>(stream), prec, tflags,
+                      synced ? &c->bn_sync : nullptr, bn_frozen))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
+}
+
+int wunet_train_forward_ex(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
+                           const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                           float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                           float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags)
+{
+    return train_forward_impl(c, x, y, B, T, conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b,
+                              momentum, workspace, workspace_bytes, stream, precision, flags, nullptr, nullptr);
+}
+
+int wunet_train_forward_blocks(wunet_ctx *c, const float *x, float *y, int B, int T, const float *const *conv_w,
+                               const float *const *conv_b, const float *const *bn_weight, const float *const *bn_bias,
+                               float *const *bn_running_mean, float *const *bn_running_var, const float *out_w, const float *out_b,
+                               float momentum, void *workspace, size_t workspace_bytes, void *stream, int precision, int flags,
+                               const unsigned char *bn_frozen, const float *momenta)
+{
+    return train_forward_impl(c, x, y, B, T, conv_w, conv_b, bn_weight, bn_bias, bn_running_mean, bn_running_var, out_w, out_b,
+                              momentum, workspace, workspace_bytes, stream, precision, flags, bn_frozen, momenta);
 }
 
 int wunet_train_backward(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
@@ -587,19 +618,22 @@ int wunet_train_backward_part_prec(wunet_ctx *c, const float *x, const float *y,
                                    g_out_w, g_out_b, workspace, workspace_bytes, stream, nullptr, part, precision, 0);
 }
 
-int wunet_train_backward_ex(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
-                            const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
-                            const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
-                            float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
-                            void *stream, float *dx, int part, int precision, int flags)
+// wunet_train_backward_ex (blocks = false: every gradient slot set unless WUNET_TRAIN_NO_PARAM_GRADS, no early stop) and
+// wunet_train_backward_blocks (null slots are frozen parameters; bn_frozen as in the forward)
+static int train_backward_impl(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
+                               const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                               const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                               float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                               void *stream, float *dx, int part, int precision, int flags, bool blocks,
+                               const unsigned char *bn_frozen)
 {
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
     const int prec = train_prec(precision);
     if (prec < 0) return WUNET_EINVAL;
     if (flags & ~kTrainFlags) return fail(WUNET_EINVAL, "unknown training flags 0x%x", flags);
-    if (dx && part == 0) return fail(WUNET_EINVAL, "dx belongs to part 1 (block 0): pass it with part -1 or 1, not 0");
-    const bool pgrads = !(flags & WUNET_TRAIN_NO_PARAM_GRADS);
+    if (dx && part == 0 && !blocks) return fail(WUNET_EINVAL, "dx belongs to part 1 (block 0): pass it with part -1 or 1, not 0");
+    const bool pgrads = !(flags & WUNET_TRAIN_NO_PARAM_GRADS) && !blocks;
     if (!x || !y || !dy || !workspace || !conv_w || !bn_weight || !bn_bias || !out_w ||
         (pgrads && (!g_conv_w || !g_conv_b || !g_bn_weight || !g_bn_bias || !g_out_w || !g_out_b)))
         return fail(WUNET_EINVAL, "null argument");
@@ -609,11 +643,36 @@ int wunet_train_backward_ex(wunet_ctx *c, const float *x, const float *y, const 
     CUDA_TRY(cudaSetDevice(c->device));
     const TrainParams P{conv_w, nullptr, bn_weight, bn_bias, nullptr, nullptr, out_w, nullptr};
     const TrainGrads G{g_conv_w, g_conv_b, g_bn_weight, g_bn_bias, g_out_w, g_out_b};
-    const bool synced = c->bn_sync.fn && !(flags & WUNET_TRAIN_FROZEN_BN);
+    bool any_batch = !(flags & WUNET_TRAIN_FROZEN_BN);
+    if (bn_frozen && any_batch) {
+        any_batch = false;
+        for (int i = 0; i < 2 * c->n + 1; ++i) any_batch = any_batch || !bn_frozen[i];
+    }
+    const bool synced = c->bn_sync.fn && any_batch;
     if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec, dx, tflags,
-                       synced ? &c->bn_sync : nullptr))
+                       synced ? &c->bn_sync : nullptr, bn_frozen, blocks))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
+}
+
+int wunet_train_backward_ex(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
+                            const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                            const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                            float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                            void *stream, float *dx, int part, int precision, int flags)
+{
+    return train_backward_impl(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight, g_bn_bias,
+                               g_out_w, g_out_b, workspace, workspace_bytes, stream, dx, part, precision, flags, false, nullptr);
+}
+
+int wunet_train_backward_blocks(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
+                                const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                                const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                                float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                                void *stream, float *dx, int part, int precision, int flags, const unsigned char *bn_frozen)
+{
+    return train_backward_impl(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight, g_bn_bias,
+                               g_out_w, g_out_b, workspace, workspace_bytes, stream, dx, part, precision, flags, true, bn_frozen);
 }
 
 int wunet_train_set_bn_allreduce(wunet_ctx *c, wunet_bn_allreduce_fn fn, void *user, double *buf, size_t capacity)

@@ -14,7 +14,9 @@
 // every block but the first (Cin = 1) run on the tensor-core kernels of wunet_train_tc.cu at that operand precision instead;
 // everything else is the same fp32 code.
 // TRAIN_FROZEN_BN (eval-mode BatchNorm: running statistics, never updated) and TRAIN_NO_PARAM_GRADS (input gradient only) only
-// change the BatchNorm arithmetic and which reductions run; the convolution-shaped passes are the same kernels. The input
+// change the BatchNorm arithmetic and which reductions run; the convolution-shaped passes are the same kernels. The same holds
+// per block (bn_frozen) and per parameter (null gradient slots), with an early stop below the lowest block that needs a
+// gradient (fine-tuning with frozen layers; DESIGN §5.4). The input
 // gradient dx is train_input_grad_kernel below (head's raw-input channel + block 0's transposed conv).
 // BnSync (nn.SyncBatchNorm over data-parallel ranks): the batch-statistics reductions are split at the cross-rank sums
 // (train_bn_sync_* kernels, a host hook between them); without it the step issues exactly the launches it always did.
@@ -820,11 +822,13 @@ size_t train_workspace_bytes(int n, int ci, int B, int T, int prec, int flags)
     return (lo.total + scratch) * sizeof(float);
 }
 
-int train_forward(int n, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum, void *workspace,
-                  cudaStream_t st, int prec, int flags, const BnSync *sync)
+int train_forward(int n, int ci, const float *x, float *y, int B, int T, const TrainParams &P, const float *momentum,
+                  void *workspace, cudaStream_t st, int prec, int flags, const BnSync *sync, const unsigned char *bn_frozen)
 {
-    const bool frozen = flags & TRAIN_FROZEN_BN;
-    if (frozen) sync = nullptr;                                     // running statistics: nothing to synchronise
+    // block i normalises by its running statistics (eval-mode container) or by batch statistics; only the latter synchronise
+    auto frozen_at = [&](int i) { return (flags & TRAIN_FROZEN_BN) || (bn_frozen && bn_frozen[i]); };
+    bool any_frozen = false;
+    for (int i = 0; i < 2 * n + 1; ++i) any_frozen = any_frozen || frozen_at(i);
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
     Layout lo;
@@ -832,8 +836,8 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
     float *ws = static_cast<float *>(workspace);
     const bool naive = train_naive() && prec == TRAIN_FP32;
     // the ones / zeros vectors serve the linear conv epilogue and, as s1 = s2 = 0, the frozen-statistics BatchNorm backward
-    if (sh[0].cout * (2 * n) > kMaxC && (!naive || frozen)) return train_fail("channel plan too wide for the training kernels (%d channels)", sh[0].cout * 2 * n);
-    if (!naive || frozen) {
+    if (sh[0].cout * (2 * n) > kMaxC && (!naive || any_frozen)) return train_fail("channel plan too wide for the training kernels (%d channels)", sh[0].cout * 2 * n);
+    if (!naive || any_frozen) {
         train_fill_kernel<<<(kMaxC + 255) / 256, 256, 0, st>>>(ws + lo.ones, 1.f, kMaxC);
         train_fill_kernel<<<(kMaxC + 255) / 256, 256, 0, st>>>(ws + lo.zeros, 0.f, kMaxC);
     }
@@ -856,7 +860,7 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
         } else if (s.mode == SRC_DIRECT) train_conv_fwd_kernel<15, SRC_DIRECT><<<grid, 128, 0, st>>>(a, P.conv_w[i], P.conv_b[i], z);
         else if (s.mode == SRC_DECIM) train_conv_fwd_kernel<15, SRC_DECIM><<<grid, 128, 0, st>>>(a, P.conv_w[i], P.conv_b[i], z);
         else train_conv_fwd_kernel<5, SRC_UPCAT><<<grid, 128, 0, st>>>(a, P.conv_w[i], P.conv_b[i], z);
-        if (frozen)
+        if (frozen_at(i))
             train_bn_frozen_stats_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(P.bn_mean[i], P.bn_var[i], ws + lo.mean[i],
                                                                                    ws + lo.invstd[i], s.cout);
         else if (sync) {
@@ -867,10 +871,10 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
             train_bn_sync_centred_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, buf);
             if (const int rc = sync->fn(sync->user, buf + s.cout + 1, (size_t)s.cout, st))
                 return train_fail("training forward, block %d: the BatchNorm all-reduce hook failed on the variances (status %d)", i, rc);
-            train_bn_sync_finalize_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(buf, s.cout, momentum, ws + lo.mean[i], ws + lo.invstd[i],
-                                                                                    P.bn_mean[i], P.bn_var[i]);
+            train_bn_sync_finalize_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(buf, s.cout, momentum[i], ws + lo.mean[i],
+                                                                                    ws + lo.invstd[i], P.bn_mean[i], P.bn_var[i]);
         } else
-            train_bn_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, momentum, ws + lo.mean[i], ws + lo.invstd[i],
+            train_bn_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(z, B, s.cout, s.L, momentum[i], ws + lo.mean[i], ws + lo.invstd[i],
                                                                      P.bn_mean[i], P.bn_var[i]);
         const long long nel = (long long)B * s.cout * s.L;
         train_bn_act_kernel<<<blocks_for(nel, 256), 256, 0, st>>>(z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
@@ -885,7 +889,7 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
 
 int train_backward(int n, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
                    const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec, float *dx, int flags,
-                   const BnSync *sync)
+                   const BnSync *sync, const unsigned char *bn_frozen, bool early_stop)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
@@ -894,74 +898,91 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
     float *ws = static_cast<float *>(workspace);
     const int last = 2 * n, C = sh[last].cout;
     const bool naive = train_naive() && prec == TRAIN_FP32;
-    const bool frozen = flags & TRAIN_FROZEN_BN, pgrads = !(flags & TRAIN_NO_PARAM_GRADS);
-    if (frozen) sync = nullptr;                                     // as in the forward
-    const bool det = pgrads && (flags & TRAIN_DETERMINISTIC);      // without parameter gradients nothing is summed atomically
+    const bool pgrads = !(flags & TRAIN_NO_PARAM_GRADS);
+    auto frozen_at = [&](int i) { return (flags & TRAIN_FROZEN_BN) || (bn_frozen && bn_frozen[i]); };
+    // the gradient slots this call fills: a null array or entry is a frozen parameter (nothing computed, nothing written)
+    auto slot = [&](float *const *g, int i) { return pgrads && g ? g[i] : nullptr; };
+    float *const g_wo = pgrads ? G.out_w : nullptr, *const g_bo = pgrads ? G.out_b : nullptr;
+    auto block_wants = [&](int i) { return slot(G.conv_w, i) || slot(G.conv_b, i) || slot(G.bn_w, i) || slot(G.bn_b, i); };
+    // early stop: j = the lowest block (the last in backward order) that still needs something — a parameter gradient or,
+    // through block 0, dx. Block j skips its input gradient; blocks below j issue nothing. Without early_stop every block runs
+    // (the _ex entry points: their split backward's part 0 cannot know whether part 1 will ask for dx).
+    int j = 0;
+    if (early_stop && !dx) {
+        j = last + 1;
+        for (int i = 0; i <= last && j > last; ++i)
+            if (block_wants(i)) j = i;
+    }
+    bool any_grad = g_wo || g_bo;
+    for (int i = 0; i <= last; ++i) any_grad = any_grad || block_wants(i);
+    const bool det = any_grad && (flags & TRAIN_DETERMINISTIC);    // without parameter gradients nothing is summed atomically
     float *scratch = ws + lo.total;                                 // TRAIN_DETERMINISTIC only (det_scratch_floats)
     if (part < -1 || part > 1) return train_fail("training backward: part must be -1, 0 or 1 (got %d)", part);
-    if (dx && part == 0) return train_fail("training backward: dx is written by part 1 (or -1), not part 0");
+    if (dx && part == 0 && !early_stop) return train_fail("training backward: dx is written by part 1 (or -1), not part 0");
     if (det && naive) return train_fail("training backward: WUNET_TRAIN_NAIVE=1 has no deterministic weight gradient");
-    if (part != 1) {
+    if (part != 1 && (g_wo || g_bo || j <= last)) {
         const unsigned hb = blocks_for((long long)B * T, 256);
-        if (det) {
+        // one head parameter frozen, the other not: the kernel computes both, the frozen one into the (idle) din region
+        float *hw = g_wo ? g_wo : ws + lo.din, *hbias = g_bo ? g_bo : ws + lo.din;
+        if (det && (g_wo || g_bo)) {
             double *hp = reinterpret_cast<double *>(scratch);
-            train_head_bwd_kernel<true><<<hb, 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last], G.out_w,
-                                                            G.out_b, hp, B, C, T);
-            train_head_sum_kernel<<<(unsigned)(C + 2), 256, 0, st>>>(hp, (int)hb, C, G.out_w, G.out_b);
+            train_head_bwd_kernel<true><<<hb, 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last], hw, hbias, hp,
+                                                            B, C, T);
+            train_head_sum_kernel<<<(unsigned)(C + 2), 256, 0, st>>>(hp, (int)hb, C, hw, hbias);
         } else {
-            if (pgrads) {
-                cudaMemsetAsync(G.out_w, 0, (C + 1) * sizeof(float), st);
-                cudaMemsetAsync(G.out_b, 0, sizeof(float), st);
+            if (g_wo || g_bo) {
+                cudaMemsetAsync(hw, 0, (C + 1) * sizeof(float), st);
+                cudaMemsetAsync(hbias, 0, sizeof(float), st);
             }
             train_head_bwd_kernel<false><<<hb, 256, 0, st>>>(dy, y, ws + lo.act[last], x, P.out_w, ws + lo.ga[last],
-                                                             pgrads ? G.out_w : nullptr, G.out_b, nullptr, B, C, T);
+                                                             (g_wo || g_bo) ? hw : nullptr, hbias, nullptr, B, C, T);
         }
     }
-    const int i_hi = (part == 1) ? n : last, i_lo = (part == 0) ? n + 1 : 0;
+    const int i_hi = (part == 1) ? n : last, i_lo = std::max((part == 0) ? n + 1 : 0, j);
     for (int i = i_hi; i >= i_lo; --i) {
         const Shape &s = sh[i];
         float *ga = ws + lo.ga[i];                               // gradient of the activation; becomes dz in place
         const float *z = ws + lo.z[i];
         const long long nel = (long long)B * s.cout * s.L;
+        float *g_gamma = slot(G.bn_w, i), *g_beta = slot(G.bn_b, i), *g_cb = slot(G.conv_b, i), *g_cw = slot(G.conv_w, i);
+        const bool frozen = frozen_at(i);
         // batch statistics: dz needs mean(dy) and mean(dy zh) (s1, s2); frozen statistics: they are constants, dz = invstd
         // gamma dy (s1 = s2 = 0), and the reductions only serve the BatchNorm parameter gradients
-        if (sync) {
+        if (sync && !frozen) {
             train_bn_sync_bwd_sums_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i],
-                                                                             P.bn_b[i], pgrads ? G.bn_w[i] : nullptr,
-                                                                             pgrads ? G.bn_b[i] : nullptr, sync->buf, B, s.cout, s.L);
+                                                                             P.bn_b[i], g_gamma, g_beta, sync->buf, B, s.cout, s.L);
             if (const int rc = sync->fn(sync->user, sync->buf, 2 * (size_t)s.cout + 1, st))
                 return train_fail("training backward, block %d: the BatchNorm all-reduce hook failed (status %d)", i, rc);
             train_bn_sync_bwd_finalize_kernel<<<blocks_for(s.cout, 256), 256, 0, st>>>(sync->buf, s.cout, ws + lo.s1[i], ws + lo.s2[i]);
-        } else if (!frozen || pgrads)
+        } else if (!frozen || g_gamma || g_beta)
             train_bn_bwd_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
-                                                                         pgrads ? G.bn_w[i] : nullptr, pgrads ? G.bn_b[i] : nullptr,
-                                                                         ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);
+                                                                         g_gamma, g_beta, ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);
         const float *s1 = frozen ? ws + lo.zeros : ws + lo.s1[i], *s2 = frozen ? ws + lo.zeros : ws + lo.s2[i];
         train_bn_bwd_apply_kernel<<<blocks_for(nel, 256), 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
                                                                         s1, s2, B, s.cout, s.L);
         const ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
-        if (pgrads) {
-            train_channel_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, G.conv_b[i], B, s.cout, s.L);
+        if (g_cb) train_channel_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, g_cb, B, s.cout, s.L);
+        if (g_cw) {
             // weight gradient: gridDim.z slices combined with atomicAdd into the zeroed dW or, in deterministic mode, stored to
             // the scratch and summed in slice order
             const long long nw = (long long)s.cout * s.cin * s.k;
-            float *wdst = det ? scratch : G.conv_w[i];
-            if (!det) cudaMemsetAsync(G.conv_w[i], 0, (size_t)nw * sizeof(float), st);
+            float *wdst = det ? scratch : g_cw;
+            if (!det) cudaMemsetAsync(g_cw, 0, (size_t)nw * sizeof(float), st);
             const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
             if (on_tc(prec, i)) {
                 if (launch_train_wgrad_tc(prec, a, ga, wdst, s.k, s.mode, st, det) < 0) return train_fail("training backward, block %d: tensor-core weight-gradient launch failed", i);
             } else if (!naive) {
                 launch_wgrad_fp32(a, ga, wdst, s.mode, st, det);
-            } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
-            else if (s.mode == SRC_DECIM) train_conv_bwd_weight_kernel<15, SRC_DECIM><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
-            else train_conv_bwd_weight_kernel<5, SRC_UPCAT><<<gw, 128, 0, st>>>(a, ga, G.conv_w[i]);
+            } else if (s.mode == SRC_DIRECT) train_conv_bwd_weight_kernel<15, SRC_DIRECT><<<gw, 128, 0, st>>>(a, ga, g_cw);
+            else if (s.mode == SRC_DECIM) train_conv_bwd_weight_kernel<15, SRC_DECIM><<<gw, 128, 0, st>>>(a, ga, g_cw);
+            else train_conv_bwd_weight_kernel<5, SRC_UPCAT><<<gw, 128, 0, st>>>(a, ga, g_cw);
             if (det) {
                 const WgradGrid g = wgrad_grid_of(prec, i, B, s.L, s.cin, s.cout, s.k);
-                train_slice_sum_kernel<<<blocks_for(nw, 256), 256, 0, st>>>(scratch, G.conv_w[i], (int)g.grid.z, nw);
+                train_slice_sum_kernel<<<blocks_for(nw, 256), 256, 0, st>>>(scratch, g_cw, (int)g.grid.z, nw);
             }
         }
-        // input gradient and its routing to the producers of the block input
-        if (s.mode != SRC_DIRECT) {
+        // input gradient and its routing to the producers of the block input (none below block j needs it)
+        if (s.mode != SRC_DIRECT && i > j) {
             float *din = ws + lo.din;
             const dim3 gd((unsigned)((s.L + 127) / 128), (unsigned)((s.cin + 7) / 8), (unsigned)B);
             if (!naive) {
@@ -980,7 +1001,9 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
                 train_decim_adjoint_kernel<<<blocks_for((long long)B * s.cin * s.L, 256), 256, 0, st>>>(din, ws + lo.ga[i - 1], B, s.cin, s.L);
             } else {
                 const int e = 2 * n - i;
-                train_skip_grad_kernel<<<blocks_for((long long)B * s.cin1 * s.L, 256), 256, 0, st>>>(din, ws + lo.ga[e], B, s.cin, s.cin0, s.L);
+                if (e >= j)
+                    train_skip_grad_kernel<<<blocks_for((long long)B * s.cin1 * s.L, 256), 256, 0, st>>>(din, ws + lo.ga[e], B, s.cin,
+                                                                                                         s.cin0, s.L);
                 train_upsample_adjoint_kernel<<<blocks_for((long long)B * s.cin0 * (s.L / 2), 256), 256, 0, st>>>(
                     din, ws + lo.ga[i - 1], B, s.cin, s.cin0, s.L, a.up_scale);
             }
@@ -988,7 +1011,7 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return train_fail("training backward, block %d: %s", i, cudaGetErrorString(e));
     }
-    if (dx) {
+    if (dx && part != 0) {
         // part -1 or 1: ga[0] now holds block 0's dz
         const dim3 gx(blocks_for(T, 256), (unsigned)B);
         train_input_grad_kernel<15><<<gx, 256, 0, st>>>(ws + lo.ga[0], P.conv_w[0], dy, y, P.out_w, dx, sh[0].cout, C, T);

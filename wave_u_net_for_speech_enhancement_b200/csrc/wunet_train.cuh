@@ -49,18 +49,25 @@ struct BnSync {
 const char *train_error();
 size_t train_workspace_bytes(int n_layers, int ci, int B, int T, int prec = TRAIN_FP32, int flags = 0);
 // y = model(x) with BatchNorm in training mode (or, with TRAIN_FROZEN_BN, eval mode); keeps every pre-BN output and
-// activation in `workspace` for the backward. sync (batch statistics only; null = this rank's frames alone): per block,
-// the local sum z and B L, hook, the local sum (z - global mean)^2, hook.
-int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, const TrainParams &P, float momentum,
-                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32, int flags = 0, const BnSync *sync = nullptr);
+// activation in `workspace` for the backward. momentum[2n+1]: each block's running-statistics factor. bn_frozen[2n+1]
+// (null = none): nonzero freezes that block's BatchNorm (running statistics, as TRAIN_FROZEN_BN does for all of them).
+// sync (batch-statistics blocks only; null = this rank's frames alone): per block, the local sum z and B L, hook, the local
+// sum (z - global mean)^2, hook.
+int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, const TrainParams &P, const float *momentum,
+                  void *workspace, cudaStream_t stream, int prec = TRAIN_FP32, int flags = 0, const BnSync *sync = nullptr,
+                  const unsigned char *bn_frozen = nullptr);
 // gradients of every parameter for the upstream gradient dy of the output; `workspace` as left by train_forward.
 // part: -1 = the whole backward; 0 = head + decoder blocks (their gradients are complete afterwards: a data-parallel caller
 // starts reducing them while part 1 runs); 1 = middle + encoder blocks (must follow part 0 on the same stream).
 // dx (optional, [B][1][T], fully overwritten): gradient of the input x; written by part -1 or 1 (block 0 is in part 1).
-// sync: must be given iff the forward had it; per block of the part, [sum dy | sum dy zh | B L], hook.
+// sync: must be given iff the forward had it; per batch-statistics block of the part, [sum dy | sum dy zh | B L], hook.
+// bn_frozen: as in the forward. A null array or entry in G is a frozen parameter: nothing is computed for it or written.
+// early_stop: nothing is issued below the lowest block that needs a gradient (or dx), and that block skips its input
+// gradient; dx then also goes to part 0, unwritten, to say that part 1 will ask for it.
 int train_backward(int n_layers, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
                    const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1, int prec = TRAIN_FP32,
-                   float *dx = nullptr, int flags = 0, const BnSync *sync = nullptr);
+                   float *dx = nullptr, int flags = 0, const BnSync *sync = nullptr, const unsigned char *bn_frozen = nullptr,
+                   bool early_stop = false);
 // One convolution-shaped pass on caller device buffers (test hook): pass 0 = forward conv out[B][Cout][L] = conv(in, w);
 // 1 = input gradient out[B][Cin][L] of dz [B][Cout][L] (Conv1d padding, no mode); 2 = weight gradient out[Cout][Cin][K] =
 // sum dz * in. `in` is built from src0 / src1 per `mode` as in the forward (ConvArgs). Synchronous.

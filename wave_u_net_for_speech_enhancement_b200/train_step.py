@@ -35,18 +35,25 @@ class GradientBucket:
 
     ``shapes``: parameter shapes in the model's ``parameters()`` order (4 per conv block — conv.weight, conv.bias, bn.weight,
     bn.bias — for the ``nblocks`` blocks in forward order, then out.weight, out.bias; model/unet_basic.py:33-75).
-    ``views[i]`` is the slice of the flat buffer that holds parameter i's gradient."""
+    ``views[i]`` is the slice of the flat buffer that holds parameter i's gradient.
 
-    def __init__(self, shapes: Sequence[torch.Size], nblocks: int, device, dtype=torch.float32):
+    ``trainable`` (optional, one bool per parameter): only these get a slot, in the same order; the others' views are None, and
+    a part with no trainable parameter is not all-reduced. Without it every parameter has one (the layout does not change)."""
+
+    def __init__(self, shapes: Sequence[torch.Size], nblocks: int, device, dtype=torch.float32,
+                 trainable: Optional[Sequence[bool]] = None):
         if len(shapes) != 4 * nblocks + 2:
             raise ValueError(f"expected {4 * nblocks + 2} parameter shapes, got {len(shapes)}")
+        if trainable is not None and len(trainable) != len(shapes):
+            raise ValueError(f"expected {len(shapes)} trainable flags, got {len(trainable)}")
+        keep = (lambda i: True) if trainable is None else (lambda i: bool(trainable[i]))     # noqa: E731
         n_enc_mid = (nblocks + 1) // 2                        # encoder blocks + middle = n + 1 of the 2n + 1 blocks
-        order: List[int] = [4 * nblocks, 4 * nblocks + 1]     # head first ...
+        order: List[int] = [i for i in (4 * nblocks, 4 * nblocks + 1) if keep(i)]      # head first ...
         for blk in range(nblocks - 1, n_enc_mid - 1, -1):     # ... decoder blocks, last to first: part 0
-            order += [4 * blk + k for k in range(4)]
+            order += [4 * blk + k for k in range(4) if keep(4 * blk + k)]
         n_part0 = len(order)
         for blk in range(n_enc_mid - 1, -1, -1):              # middle, encoder blocks last to first: part 1
-            order += [4 * blk + k for k in range(4)]
+            order += [4 * blk + k for k in range(4) if keep(4 * blk + k)]
         sizes = [int(torch.Size(shapes[i]).numel()) for i in order]
         pad = lambda n, a: (n + a - 1) // a * a             # noqa: E731 - every gradient starts 16-byte aligned
         offs, off = [], 0
@@ -56,6 +63,8 @@ class GradientBucket:
                 self.split = off
             offs.append(off)
             off += pad(n, 4)
+        if n_part0 == len(order):                            # no trainable parameter in part 1
+            self.split = off
         self.flat = torch.zeros(off, dtype=dtype, device=device)      # zeros: the padding takes part in the all-reduce
         self.views: List[Optional[torch.Tensor]] = [None] * len(shapes)
         for i, n, o in zip(order, sizes, offs):
@@ -69,7 +78,7 @@ class GradientBucket:
     def reduce_part(self, k: int, group=None) -> None:
         """Start averaging part k over the ranks (asynchronous: the collective is ordered after the work already enqueued
         on the current stream and overlaps what is enqueued next)."""
-        if data_parallel_world() == 1:
+        if data_parallel_world() == 1 or self.part(k).numel() == 0:
             return
         backend = dist.get_backend(group)
         if backend == "nccl":

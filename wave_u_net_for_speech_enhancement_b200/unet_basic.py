@@ -21,6 +21,7 @@ There is no CPU or PyTorch fallback for the eval forward: a CPU tensor or a miss
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import threading
 from typing import Dict, Optional, Tuple
@@ -166,6 +167,11 @@ class _NativeTrainStep(torch.autograd.Function):
     workspace tensor kept on the autograd context; parameter order: 4 per conv block (conv.weight, conv.bias, bn.weight,
     bn.bias) in forward order, then out.weight, out.bias.
 
+    ``blocks``: None (every BatchNorm in the mode ``flags`` says, one momentum, parameters all trainable or all frozen), or
+    ``(bn_frozen, momenta)``, the per-block lists of a fine-tuning state: the step then runs wunet_train_forward_blocks /
+    wunet_train_backward_blocks, and the backward computes only the gradients of the parameters that require grad (the
+    others get None, and the gradient bucket holds only the trainable ones).
+
     ``flags``: 0 = BatchNorm with batch statistics, running buffers updated (.train()); ``_lib.TRAIN_FROZEN_BN`` = BatchNorm
     normalising by the running statistics, which stay untouched (.eval()); either may add ``_lib.TRAIN_DETERMINISTIC`` (weight
     and head gradients summed in a fixed order, with a larger workspace). The backward fills the gradient of ``x`` when it
@@ -177,10 +183,10 @@ class _NativeTrainStep(torch.autograd.Function):
 
     @staticmethod
     def _ptr_array(tensors):
-        return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
+        return (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
 
     @staticmethod
-    def forward(ctx, model, flags, reducer, x, *params):
+    def forward(ctx, model, flags, reducer, blocks_state, x, *params):
         lib = _lib.load()
         blocks = model._blocks()
         nb = len(blocks)
@@ -199,19 +205,27 @@ class _NativeTrainStep(torch.autograd.Function):
             bn_b = [params[4 * i + 3] for i in range(nb)]
             rmean = [blk[1].running_mean for blk in blocks]
             rvar = [blk[1].running_var for blk in blocks]
-            momentum = float(blocks[0][1].momentum)
             stream = torch.cuda.current_stream(x.device).cuda_stream
             P = _NativeTrainStep._ptr_array
             # [sum dy | sum dy zhat | B L] of the widest block (n ci channels): the hook's exchange buffer
             bn_buf = None if reducer is None else torch.empty(2 * model.n_layers * model.channels_interval + 1,
                                                               dtype=torch.float64, device=x.device)
-            _native_call(lib, c, reducer, bn_buf, lambda: lib.wunet_train_forward_ex(
-                c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b), P(rmean), P(rvar),
-                params[-2].data_ptr(), params[-1].data_ptr(), momentum, ws.data_ptr(), ws.numel(), stream, prec, flags))
+            args = (c, x.data_ptr(), y.data_ptr(), B, T, P(conv_w), P(conv_b), P(bn_w), P(bn_b), P(rmean), P(rvar),
+                    params[-2].data_ptr(), params[-1].data_ptr())
+            bn_frozen = None
+            if blocks_state is None:
+                momentum = next((float(blk[1].momentum) for blk in blocks if blk[1].momentum is not None), 0.1)
+                _native_call(lib, c, reducer, bn_buf, lambda: lib.wunet_train_forward_ex(
+                    *args, momentum, ws.data_ptr(), ws.numel(), stream, prec, flags))
+            else:
+                frozen, momenta = blocks_state
+                bn_frozen = (ctypes.c_ubyte * nb)(*[1 if f else 0 for f in frozen])
+                _native_call(lib, c, reducer, bn_buf, lambda: lib.wunet_train_forward_blocks(
+                    *args, 0.0, ws.data_ptr(), ws.numel(), stream, prec, flags, bn_frozen, (ctypes.c_float * nb)(*momenta)))
         # the backward runs at the precision, BatchNorm mode and synchronisation of ITS forward (and reads the bf16 weight
         # packings that forward left in ws)
         ctx.model, ctx.ws, ctx.nb, ctx.prec, ctx.flags = model, ws, nb, prec, flags
-        ctx.reducer, ctx.bn_buf = reducer, bn_buf
+        ctx.reducer, ctx.bn_buf, ctx.bn_frozen = reducer, bn_buf, bn_frozen
         ctx.save_for_backward(x, y, *params)
         return y
 
@@ -223,14 +237,17 @@ class _NativeTrainStep(torch.autograd.Function):
         nb = ctx.nb
         B, _, T = x.shape
         gy = gy.contiguous()
-        want_dx = ctx.needs_input_grad[3]
-        want_params = any(ctx.needs_input_grad[4:])
+        want_dx = ctx.needs_input_grad[4]
+        mask = ctx.needs_input_grad[5:]
+        want_params = any(mask)
+        per_block = ctx.bn_frozen is not None              # the forward ran wunet_train_forward_blocks
         dx = torch.empty_like(x) if want_dx else None
         flags = ctx.flags | (0 if want_params else _lib.TRAIN_NO_PARAM_GRADS)
         if want_params:
             # all gradients live in ONE flat buffer laid out in backward-completion order (train_step.GradientBucket); autograd
-            # hands the views to .grad, so the all-reduce below needs no gather / scatter copies
-            bucket = GradientBucket([p.shape for p in params], nb, x.device)
+            # hands the views to .grad, so the all-reduce below needs no gather / scatter copies. Frozen parameters have no
+            # slot (None: nothing is computed for them)
+            bucket = GradientBucket([p.shape for p in params], nb, x.device, trainable=None if all(mask) else mask)
             grads = bucket.views
             reduce = ctx.model.data_parallel != "off" and data_parallel_world() > 1
         else:
@@ -243,17 +260,23 @@ class _NativeTrainStep(torch.autograd.Function):
             G = (lambda k: P(sel(grads, k))) if want_params else (lambda k: None)   # noqa: E731
             ptr = lambda t: None if t is None else t.data_ptr()               # noqa: E731
             for part in ((0, 1) if reduce else (-1,)):
-                _native_call(lib, c, ctx.reducer, ctx.bn_buf, lambda: lib.wunet_train_backward_ex(
-                    c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)), P(sel(params, 2)), P(sel(params, 3)),
-                    params[-2].data_ptr(), G(0), G(1), G(2), G(3), ptr(grads[-2]), ptr(grads[-1]), ctx.ws.data_ptr(),
-                    ctx.ws.numel(), stream, ptr(dx) if part != 0 else None, part, ctx.prec, flags))
+                args = (c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)), P(sel(params, 2)), P(sel(params, 3)),
+                        params[-2].data_ptr(), G(0), G(1), G(2), G(3), ptr(grads[-2]), ptr(grads[-1]), ctx.ws.data_ptr(),
+                        ctx.ws.numel(), stream)
+                if per_block:
+                    # dx goes to part 0 as well: it tells the early stop that part 1 will need the gradient of block 0
+                    _native_call(lib, c, ctx.reducer, ctx.bn_buf, lambda: lib.wunet_train_backward_blocks(
+                        *args, ptr(dx), part, ctx.prec, flags, ctx.bn_frozen))
+                else:
+                    _native_call(lib, c, ctx.reducer, ctx.bn_buf, lambda: lib.wunet_train_backward_ex(
+                        *args, ptr(dx) if part != 0 else None, part, ctx.prec, flags))
                 if reduce:
                     # head + decoder gradients are final after part 0: their all-reduce overlaps part 1 (middle + encoders)
                     bucket.reduce_part(part)
             if reduce:
                 bucket.finish()
-        ctx.ws = ctx.bn_buf = ctx.reducer = None
-        return (None, None, None, dx, *grads)                # no gradient for the model handle, the flags and the reducer
+        ctx.ws = ctx.bn_buf = ctx.reducer = ctx.bn_frozen = None
+        return (None, None, None, None, dx, *grads)          # none for the model handle, the flags, the reducer, the block state
 
 
 class Model(nn.Module):
@@ -315,6 +338,16 @@ class Model(nn.Module):
     ``torch.distributed`` is initialised and the containers' process group has more than one rank, as ``nn.SyncBatchNorm``
     does (three small all-reduces per block, on the current stream). The running statistics then agree on every rank, and
     with equal shards the data-parallel step equals the single-process step on the concatenated batch.
+
+    Fine-tuning with frozen layers (no constructor argument): the native step honours each BatchNorm container's own
+    ``.training`` (batch statistics, or the running statistics left untouched), ``momentum`` (``None``: the cumulative
+    factor ``1 / num_batches_tracked``) and ``num_batches_tracked``, and each parameter's ``requires_grad``: a frozen
+    parameter gets no gradient and costs no weight-gradient pass or all-reduce, and the backward stops below the lowest block
+    that still needs a gradient. So ``model.train()``, ``m.eval()`` on every ``nn.BatchNorm1d`` and
+    ``model.encoder.requires_grad_(False)`` compute what the reference computes. An ``.eval()`` model with a container in
+    ``.train()`` runs the training kernels (detached unless ``eval_autograd`` records a graph); ``forward_host`` and
+    ``forward_host_stream`` refuse it. Not supported: BatchNorm with ``affine=False`` or ``track_running_stats=False``, or an
+    ``eps`` other than the library's 1e-5.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
@@ -431,13 +464,29 @@ class Model(nn.Module):
                 "train_backend='native' (default; sm_90a kernels) or 'torch' (composite PyTorch path).")
         # eval mode: a forward that needs a graph (see eval_autograd: the input requires grad, or "always" and a parameter
         # does) runs the training kernels with eval-mode BatchNorm, or the composite path for train_backend="torch".
+        # A BatchNorm container switched back to .train() needs batch statistics, which only the training kernels compute:
+        # that forward takes them too, per-block modes, and returns a detached tensor unless it records a graph.
         # Everything else — enhancement.py:66 (`model(chunk).detach().cpu()`, no torch.no_grad()), validation under
         # torch.no_grad(), an empty batch — takes the inference kernels and gets a detached result.
-        if input.numel() != 0 and self._eval_records_graph(input):
-            if self.train_backend == "native":
-                return self._forward_train_native(input, frozen_bn=True)
-            return self._forward_torch_reference_semantics(input)
+        if input.numel() != 0:
+            records = self._eval_records_graph(input)
+            if self._bn_any_training():
+                if self.train_backend == "none":
+                    raise NotImplementedError(
+                        "a BatchNorm container of this eval-mode model is in training mode, which needs the training kernels: "
+                        "construct the model with train_backend='native' (default) or 'torch', or call .eval() on it")
+                with contextlib.nullcontext() if records else torch.no_grad():
+                    if self.train_backend == "native":
+                        return self._forward_train_native(input)
+                    return self._forward_torch_reference_semantics(input)
+            if records:
+                if self.train_backend == "native":
+                    return self._forward_train_native(input)
+                return self._forward_torch_reference_semantics(input)
         return self._forward_native(input)
+
+    def _bn_any_training(self) -> bool:
+        return any(blk[1].training for blk in self._blocks())
 
     def _eval_records_graph(self, x: torch.Tensor) -> bool:
         if self.eval_autograd == "off" or self.train_backend == "none" or not torch.is_grad_enabled():
@@ -453,17 +502,21 @@ class Model(nn.Module):
         return ((self.training or self.eval_autograd != "off") and self.train_backend == "native"
                 and self.data_parallel != "off" and data_parallel_world() > 1)
 
-    def _forward_train_native(self, x: torch.Tensor, frozen_bn: bool = False) -> torch.Tensor:
+    def _forward_train_native(self, x: torch.Tensor) -> torch.Tensor:
         """Training-kernel forward through libwunet_b200 (wunet_train_forward_ex / wunet_train_backward_ex behind a
-        torch.autograd.Function): ``loss.backward()`` fills ``.grad`` of the parameters that require grad (all 102 in
-        training) and of ``x`` when it requires grad; the caller's optimizer is used unchanged (trainer/trainer.py:34-38).
-        BatchNorm uses batch statistics and updates its running buffers (.train()) or, with ``frozen_bn``, normalises by the
-        running statistics and leaves them and ``num_batches_tracked`` untouched (.eval()). fp32 or, with
-        ``train_precision="bf16"`` / ``"tf32"``, bf16 / tf32 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
+        torch.autograd.Function): ``loss.backward()`` fills ``.grad`` of the parameters that require grad and of ``x`` when it
+        requires grad; the caller's optimizer is used unchanged (trainer/trainer.py:34-38). Each block's BatchNorm follows
+        its own container, as the reference's sub-modules do: in .train() it uses batch statistics and updates its running
+        buffers with its own momentum (None: the cumulative factor 1 / num_batches_tracked) and counter; in .eval() it
+        normalises by the running statistics and leaves them untouched. fp32 or, with ``train_precision="bf16"`` /
+        ``"tf32"``, bf16 / tf32 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
         B, _, T = x.shape
-        reducer = None if frozen_bn else self._bn_sync_reducer()
-        if not frozen_bn and reducer is None and B * (T >> self.n_layers) == 1:
+        blocks = self._blocks()
+        bns = [blk[1] for blk in blocks]
+        training = [bn.training for bn in bns]
+        reducer = self._bn_sync_reducer() if any(training) else None
+        if training[self.n_layers] and reducer is None and B * (T >> self.n_layers) == 1:
             # torch.nn.BatchNorm1d in training mode refuses batch statistics of one value per channel (here: the middle
             # block of a single frame of 2^n_layers samples); the reference raises this from self.middle
             raise ValueError("Expected more than 1 value per channel when training, got input size "
@@ -471,7 +524,6 @@ class Model(nn.Module):
         if not x.is_cuda:
             raise RuntimeError("wave_u_net_for_speech_enhancement_b200 has no CPU fallback: move the model and the "
                                "input to a CUDA (sm_90a) device")
-        blocks = self._blocks()
         params = []
         for blk in blocks:
             params += [blk[0].weight, blk[0].bias, blk[1].weight, blk[1].bias]
@@ -479,14 +531,24 @@ class Model(nn.Module):
         for t in params:
             if t.device != x.device or t.dtype != torch.float32 or not t.is_contiguous():
                 raise RuntimeError("libwunet_b200 needs contiguous float32 parameters on the input's device")
-        flags = _lib.TRAIN_FROZEN_BN if frozen_bn else 0
+        # torch.nn.BatchNorm1d's exponential_average_factor of this step: momentum, or 1 / num_batches_tracked after the
+        # increment when momentum is None (frozen blocks: unused)
+        momenta = [0.0 if not tr else 1.0 / (int(bn.num_batches_tracked) + 1) if bn.momentum is None else float(bn.momentum)
+                   for bn, tr in zip(bns, training)]
+        train_momenta = {bn.momentum for bn, tr in zip(bns, training) if tr}
+        trainable = [p.requires_grad for p in params]
+        uniform = (all(training) or not any(training)) and len(train_momenta) <= 1 and None not in train_momenta and (
+            all(trainable) or not any(trainable))
+        flags = 0 if any(training) else _lib.TRAIN_FROZEN_BN
         if torch.backends.cudnn.deterministic or torch.are_deterministic_algorithms_enabled():
             flags |= _lib.TRAIN_DETERMINISTIC
-        y = _NativeTrainStep.apply(self, flags, reducer, self._aligned(x), *params)
-        if frozen_bn:
+        blocks_state = None if uniform else ([not tr for tr in training], momenta)
+        y = _NativeTrainStep.apply(self, flags, reducer, blocks_state, self._aligned(x), *params)
+        if not any(training):
             return y                                         # running statistics untouched: the folded copies stay valid
-        for blk in blocks:                                   # torch.nn.BatchNorm1d bookkeeping (momentum is not None: unused)
-            blk[1].num_batches_tracked += 1
+        for bn, tr in zip(bns, training):                    # torch.nn.BatchNorm1d bookkeeping
+            if tr:
+                bn.num_batches_tracked += 1
         # the kernels updated running_mean / running_var through raw pointers (no _version bump): drop the folded copies
         self._native.invalidate_weights()
         return y
@@ -567,8 +629,8 @@ class Model(nn.Module):
         self._check_input(x_host)
         if x_host.is_cuda:
             raise RuntimeError("forward_host takes a host tensor")
-        if self.training:
-            raise NotImplementedError("forward_host is eval-only")
+        if self.training or self._bn_any_training():
+            raise NotImplementedError("forward_host is eval-only (model and every BatchNorm container in .eval())")
         empty = self._empty_batch(x_host)
         if empty is not None:
             return empty if out is None else out
@@ -594,8 +656,8 @@ class Model(nn.Module):
         yields one output tensor per input batch, in order; H2D copy, kernels and D2H copy of consecutive batches overlap
         (two batches in flight). ``batches``: iterable of pinned ``[B,1,T]`` float32 host tensors that must stay alive until
         their result has been yielded; ``outs``: optional iterable of pinned output tensors."""
-        if self.training:
-            raise NotImplementedError("forward_host_stream is eval-only")
+        if self.training or self._bn_any_training():
+            raise NotImplementedError("forward_host_stream is eval-only (model and every BatchNorm container in .eval())")
         device = self.out[0].weight.device
         if device.type != "cuda":
             raise RuntimeError("no CPU fallback: move the model to a CUDA device first")
