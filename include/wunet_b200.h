@@ -47,6 +47,9 @@ extern "C" {
                                interpolates in packed fp16 and forms b - a of two adjacent values: more than 65504 apart -> inf.
                                Same workspace and tiling plan as WUNET_PREC_BF16; block 0 stays on the CUDA cores (WUNET_TC_ENC0
                                does not apply). The training entry points reject it (WUNET_EINVAL). */
+#define WUNET_PREC_FP16_SCALED 5 /* training step only: fp16 operands (round to nearest even, no saturation) with per-block
+                               power-of-two scaling of dz, fp32 accumulate on wgmma tensor cores (see the training entry points);
+                               the inference entry points reject it (WUNET_EINVAL) */
 
 typedef struct wunet_ctx wunet_ctx;
 
@@ -215,6 +218,17 @@ int wunet_train_backward_part(wunet_ctx *ctx, const float *x, const float *y, co
  *                    nearest, ties away from zero: cvt.rna.tf32.f32) and the products are accumulated in fp32 on wgmma
  *                    (m64nNk8.f32.tf32.tf32). This is the arithmetic of cuDNN's Conv1d with torch.backends.cudnn.allow_tf32
  *                    (PyTorch's default), i.e. of the reference's own training step on an H100. The first block stays fp32.
+ *   WUNET_PREC_FP16_SCALED  the same mixed-precision contract with fp16 operands (round to nearest even; beyond +-65504 they
+ *                    become +-inf and NaN stays NaN: unlike the inference fp16 stores nothing saturates, so a non-finite
+ *                    value reaches the gradients, e.g. a GradScaler's found_inf, instead of being hidden) and per-block scaling
+ *                    of dz, which fp16's range could not hold unscaled: for each block j the backward finds amax_j = max |dz_j|
+ *                    on the device and k_j with amax_j 2^k_j in [2^13, 2^14) (k_j = 0 when amax_j is 0 or not finite; |k_j| <=
+ *                    126); the input and weight gradients use fp16(dz 2^k_j) and their results are multiplied by 2^-k_j.
+ *                    Powers of two are exact in fp32, so each pass computes exactly sum fp16(dz 2^k) fp16(x) 2^-k, and the
+ *                    gradients of loss 2^m are 2^m times those of loss. The forward operands are not scaled. No host sync: the
+ *                    step stays graph-capturable and, with WUNET_TRAIN_DETERMINISTIC, bitwise repeatable (max is
+ *                    order-independent). Each data-parallel rank picks its own k_j. The first block stays fp32. The workspace
+ *                    is the WUNET_PREC_BF16 one (fp16 packings take the bytes of the bf16 ones) plus 2 n_layers + 1 scale slots.
  *   WUNET_PREC_FP32_TC, WUNET_PREC_FP16 -> WUNET_EINVAL (not training precisions).
  * The backward must use the precision and workspace of its forward. Same call sites as above (trainer/trainer.py:35-37). */
 size_t wunet_train_workspace_bytes_prec(const wunet_ctx *ctx, int B, int T, int precision);
@@ -318,7 +332,8 @@ typedef int (*wunet_bn_allreduce_fn)(void *user, double *buf, size_t count, void
 int wunet_train_set_bn_allreduce(wunet_ctx *ctx, wunet_bn_allreduce_fn fn, void *user, double *buf, size_t capacity);
 
 /* Test hook, synchronous, on caller device buffers (fp32): one convolution-shaped pass of the training step at `precision`
- * (WUNET_PREC_FP32, WUNET_PREC_BF16 or WUNET_PREC_TF32), the kernels the step itself uses. mode: 0 = direct, 1 = decimated (src0 is
+ * (WUNET_PREC_FP32, WUNET_PREC_BF16, WUNET_PREC_TF32 or WUNET_PREC_FP16_SCALED), the kernels the step itself uses (at
+ * WUNET_PREC_FP16_SCALED passes 1 and 2 scale dz by 2^k of its max |dz|, as the step does per block). mode: 0 = direct, 1 = decimated (src0 is
  * [B][cin0][2L], every other sample read), 2 = upsample + concat (src0 = [B][cin0][L/2] interpolated 2x linearly,
  * align_corners=True, then src1 = [B][cin1][L]); ksize 15 with modes 0/1, 5 with mode 2 (pass 1 also takes 5 with mode 0).
  * w = [cout][cin0 + cin1][ksize] (Conv1d, no bias).
@@ -330,20 +345,25 @@ int wunet_debug_train_conv(int pass, int precision, int mode, int ksize, int B, 
                            const float *src0, const float *src1, const float *w, const float *dz, float *out);
 
 /* Introspection for tests, host-only (needs no GPU, no context): the training step of an n_layers / channels_interval model at
- * batch B, frame length T and training `precision` (WUNET_PREC_FP32, _BF16 or _TF32), block `block` (0 .. 2*n_layers, forward
- * order). Writes 22 long longs (capacity >= 22):
+ * batch B, frame length T and training `precision` (WUNET_PREC_FP32, _BF16, _TF32 or _FP16_SCALED), block `block` (0 .. 2*n_layers,
+ * forward order). Writes 22 long longs (capacity >= 22), and a 23rd when capacity >= 23:
  *  [0] z  [1] act  [2] ga  [3] mean  [4] invstd  [5] s1  [6] s2: byte offsets in the training workspace of the block's pre-BatchNorm
  *      output z [B][Cout][L], its activation [B][Cout][L], the activation gradient [B][Cout][L] (which holds dz after the
  *      backward), and the fp32 [Cout] vectors of the BatchNorm mean and 1/sqrt(var + eps) used by the forward and of the
  *      backward's mean(dy) and mean(dy * zhat) (written when that reduction runs)
  *  [7] Cin  [8] Cin0  [9] Cin1 (the skip channels of a decoder)  [10] Cout  [11] L  [12] ksize  [13] input mode (0 = the raw input,
  *      1 = the previous activation decimated, 2 = interpolated previous activation + skip)
- *  [14] weight-gradient kernel (0 = fp32 tiled, 1 = bf16 wgmma, 2 = tf32 wgmma; block 0 is always 0)  [15] [16] [17] its gridDim x, y, z
+ *  [14] weight-gradient kernel (0 = fp32 tiled, 1 = bf16 wgmma, 2 = tf32 wgmma, 3 = fp16 wgmma; block 0 is always 0)  [15] [16] [17] its gridDim x, y, z
  *  [18] (frame, position tile) work items shared by the gridDim.z slices  [19] positions per item  [20] largest number of items
- *      one CTA reduces  [21] wunet_train_workspace_bytes_prec for this B, T and precision.
+ *      one CTA reduces  [21] wunet_train_workspace_bytes_prec for this B, T and precision
+ *  [22] WUNET_PREC_FP16_SCALED: byte offset of the block's dz scale slot (one float: max |dz| of the block, written by the
+ *      backward); -1 for other precisions and for block 0.
  * No reference counterpart. */
 int wunet_debug_train_layout(int n_layers, int channels_interval, int B, int T, int precision, int block, long long *fields,
                              int capacity);
+/* Host-only (needs no GPU): the k of WUNET_PREC_FP16_SCALED's dz scaling for a block whose max |dz| is amax: amax 2^k in
+ * [2^13, 2^14); 0 when amax is 0, NaN or infinite; clamped to [-126, 126]. The kernels use the same function. */
+int wunet_debug_train_dz_scale(float amax);
 
 /* Introspection for tests and tuning, host-only (needs no GPU, no context): the tiling the bf16 path would use for conv
  * block `block` (1 .. 2*n_layers; block 0 = first encoder runs on CUDA cores) at batch B, frame length T, on a device with

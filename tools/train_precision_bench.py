@@ -1,9 +1,11 @@
-"""Training-step time of the reference architecture (n_layers 12, channels_interval 24, T = 16384) in eight legs:
+"""Training-step time of the reference architecture (n_layers 12, channels_interval 24, T = 16384) in ten legs:
 
     native fp32   Model(train_backend="native", train_precision="fp32")   fp32 FFMA convolutions (wunet_train.cu)
     native bf16   Model(train_backend="native", train_precision="bf16")   bf16 wgmma convolutions (wunet_train_tc.cu)
     native tf32   Model(train_backend="native", train_precision="tf32")   tf32 wgmma convolutions (wunet_train_tc.cu)
-    *_det         the same three under torch.backends.cudnn.deterministic = True: deterministic mode (ordered weight- and
+    native fp16_scaled  Model(train_backend="native", train_precision="fp16_scaled")   fp16 wgmma convolutions with per-block
+                  dz scaling (wunet_train_tc_f16.cu)
+    *_det         the same four under torch.backends.cudnn.deterministic = True: deterministic mode (ordered weight- and
                   head-gradient sums instead of float atomics)
     autocast      Model(train_backend="torch") under torch.autocast("cuda", torch.bfloat16): PyTorch eager + cuDNN
     eager_tf32    Model(train_backend="torch") in fp32 with torch.backends.cudnn.allow_tf32 = True: PyTorch eager + cuDNN's
@@ -41,6 +43,8 @@ LEGS = {
     "native_bf16_det": dict(train_backend="native", train_precision="bf16"),
     "native_tf32": dict(train_backend="native", train_precision="tf32"),
     "native_tf32_det": dict(train_backend="native", train_precision="tf32"),
+    "native_fp16_scaled": dict(train_backend="native", train_precision="fp16_scaled"),
+    "native_fp16_scaled_det": dict(train_backend="native", train_precision="fp16_scaled"),
     "autocast_bf16": dict(train_backend="torch"),
     "eager_tf32": dict(train_backend="torch"),
 }
@@ -132,7 +136,7 @@ def main():
             for leg in legs:
                 r = run_steps(leg, states[leg], a.steps, timed=True)
                 runs[leg].append(r)
-                print(f"B={B} rep {rep} {leg:14s} step {r['step_ms']:8.2f} ms (fwd {r['forward_ms']:.2f}, bwd {r['backward_ms']:.2f}, "
+                print(f"B={B} rep {rep} {leg:22s} step {r['step_ms']:8.2f} ms (fwd {r['forward_ms']:.2f}, bwd {r['backward_ms']:.2f}, "
                       f"adam {r['adam_ms']:.2f}; wall {r['wall_step_ms']:.2f})", flush=True)
         summary = {}
         for leg in legs:

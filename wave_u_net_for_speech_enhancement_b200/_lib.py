@@ -12,8 +12,10 @@ PREC_BF16 = 1
 PREC_FP32_TC = 2
 PREC_TF32 = 3
 PREC_FP16 = 4
+PREC_FP16_SCALED = 5
 PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC, "fp16": PREC_FP16}   # inference (Model(precision=...))
-TRAIN_PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32}      # training step (Model(train_precision=...))
+TRAIN_PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32,      # training step (Model(train_precision=...))
+                    "fp16_scaled": PREC_FP16_SCALED}
 
 TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mode BatchNorm
 TRAIN_NO_PARAM_GRADS = 2   # backward: input gradient only
@@ -86,6 +88,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_set_bn_allreduce.argtypes = [vp, BN_ALLREDUCE_FN, vp, vp, cs]
     lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     lib.wunet_debug_train_layout.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ll), ci]
+    lib.wunet_debug_train_dz_scale.argtypes = [ctypes.c_float]
     _lib = lib
     return lib
 
@@ -103,7 +106,7 @@ EXPORTED_SYMBOLS = [
     "wunet_train_workspace_bytes", "wunet_train_forward", "wunet_train_backward", "wunet_train_backward_part",
     "wunet_train_workspace_bytes_prec", "wunet_train_forward_prec", "wunet_train_backward_part_prec", "wunet_debug_train_conv",
     "wunet_train_forward_ex", "wunet_train_backward_ex", "wunet_train_workspace_bytes_ex", "wunet_debug_train_layout",
-    "wunet_train_set_bn_allreduce", "wunet_train_forward_blocks", "wunet_train_backward_blocks",
+    "wunet_train_set_bn_allreduce", "wunet_train_forward_blocks", "wunet_train_backward_blocks", "wunet_debug_train_dz_scale",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
 ]

@@ -300,6 +300,8 @@ size_t wunet_workspace_bytes(const wunet_ctx *c, int B, int T, int precision)
     }
     if (tc_mode(precision) >= 0) return tc_workspace_bytes(c->n, c->ci, B, T, tc_mode(precision));
     if (precision == WUNET_PREC_TF32) fail(WUNET_EINVAL, "WUNET_PREC_TF32 is a training precision only (the forward has no tf32 path)");
+    else if (precision == WUNET_PREC_FP16_SCALED)
+        fail(WUNET_EINVAL, "WUNET_PREC_FP16_SCALED is a training precision only (inference in fp16 is WUNET_PREC_FP16)");
     else fail(WUNET_EINVAL, "unknown precision %d", precision);
     return 0;
 }
@@ -468,8 +470,10 @@ static int train_prec(int precision)
     if (precision == WUNET_PREC_FP32) return TRAIN_FP32;
     if (precision == WUNET_PREC_BF16) return TRAIN_BF16;
     if (precision == WUNET_PREC_TF32) return TRAIN_TF32;
+    if (precision == WUNET_PREC_FP16_SCALED) return TRAIN_FP16_SCALED;
     if (precision == WUNET_PREC_FP32_TC || precision == WUNET_PREC_FP16)
-        fail(WUNET_EINVAL, "training precision %s is not supported: use WUNET_PREC_FP32, WUNET_PREC_BF16 or WUNET_PREC_TF32",
+        fail(WUNET_EINVAL, "training precision %s is not supported: use WUNET_PREC_FP32, WUNET_PREC_BF16, WUNET_PREC_TF32 or "
+             "WUNET_PREC_FP16_SCALED",
              precision == WUNET_PREC_FP16 ? "WUNET_PREC_FP16" : "WUNET_PREC_FP32_TC");
     else
         fail(WUNET_EINVAL, "unknown training precision %d", precision);
@@ -710,6 +714,8 @@ int wunet_debug_train_layout(int n_layers, int channels_interval, int B, int T, 
         return fail(WUNET_EINVAL, "%s", train_error());
     return WUNET_OK;
 }
+
+int wunet_debug_train_dz_scale(float amax) { return dz_scale_exp(amax); }
 
 int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity)
 {

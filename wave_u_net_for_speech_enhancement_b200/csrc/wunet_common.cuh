@@ -75,8 +75,9 @@ int launch_pack_fp32(const float *w, const float *bias, const float *g, const fl
                      cudaStream_t st);
 
 // ---- tensor-core training convolutions, implemented in wunet_train_tc.cu ------------------------------------------------
-// prec (TrainPrec, wunet_train.cuh) is TRAIN_BF16 (bf16 operands, round to nearest) or TRAIN_TF32 (tf32 operands, round to
-// nearest, ties away: cvt.rna.tf32.f32); products are accumulated in fp32.
+// prec (TrainPrec, wunet_train.cuh) is TRAIN_BF16 (bf16 operands, round to nearest), TRAIN_TF32 (tf32 operands, round to
+// nearest, ties away: cvt.rna.tf32.f32) or TRAIN_FP16_SCALED (fp16 operands, round to nearest even; dz staged at its block's
+// power-of-two scale, wunet_train_tc_kernels.cuh); products are accumulated in fp32.
 // launch_train_conv_tc: launch_conv_fp32's operator with a.wp pointing at the forward (or input-gradient) packing written by
 // train_tc_pack at the same precision; ksize 15 (DIRECT, DECIM) or 5 (DIRECT, UPCAT).
 int launch_train_conv_tc(int prec, const ConvArgs &a, int ksize, int mode, cudaStream_t st);
@@ -88,9 +89,13 @@ int launch_train_wgrad_tc(int prec, const ConvArgs &a, const float *dz, float *d
 // grid, number of (frame, position tile) work items that gridDim.z slices share, and positions per item.
 struct WgradGrid { dim3 grid; int items, positions; };
 WgradGrid wgrad_grid_fp32(int B, int L, int Cin, int Cout);             // train_wgrad_kernel (wunet_train.cu)
-WgradGrid wgrad_grid_tc(int B, int L, int Cin, int Cout, int ksize);    // the tensor-core ones, at both precisions
+WgradGrid wgrad_grid_tc(int B, int L, int Cin, int Cout, int ksize);    // the tensor-core ones, at every precision
 // bytes of one packing of a [cout][cin][k] weight (forward: (cout, cin); input gradient: (cin, cout)); a multiple of 256
 size_t train_tc_packed_bytes(int prec, int cout, int cin, int k);
 int train_tc_pack(int prec, const float *w, void *wf, void *wb, int Cout, int Cin, int K, cudaStream_t st);
+// the TRAIN_FP16_SCALED instances of the three (wunet_train_tc_f16.cu)
+int train_tc_pack_f16(const float *w, void *wf, void *wb, int Cout, int Cin, int K, cudaStream_t st);
+int launch_train_conv_tc_f16(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
+int launch_train_wgrad_tc_f16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices);
 
 }  // namespace wunet

@@ -10,9 +10,11 @@
 // scratch region after the workspace layout and summed in an order fixed by the shapes (train_slice_sum_kernel,
 // train_head_sum_kernel); every other reduction of the step already has a fixed order.
 // The naive one-thread-per-output kernels they replace are kept as WUNET_TRAIN_NAIVE=1 (cross-check, tests).
-// TRAIN_BF16 / TRAIN_TF32 (Model(train_precision="bf16" / "tf32")): the forward conv, input gradient and weight gradient of
-// every block but the first (Cin = 1) run on the tensor-core kernels of wunet_train_tc.cu at that operand precision instead;
-// everything else is the same fp32 code.
+// TRAIN_BF16 / TRAIN_TF32 / TRAIN_FP16_SCALED (Model(train_precision="bf16" / "tf32" / "fp16_scaled")): the forward conv,
+// input gradient and weight gradient of every block but the first (Cin = 1) run on the tensor-core kernels of
+// wunet_train_tc_kernels.cuh at that operand precision instead; everything else is the same fp32 code. TRAIN_FP16_SCALED adds
+// one reduction per block: the BatchNorm backward that writes dz also finds max |dz| (train_bn_bwd_apply_amax_kernel), from
+// which the two passes that read dz take its power-of-two scale on the device (no host sync; max is order-independent).
 // TRAIN_FROZEN_BN (eval-mode BatchNorm: running statistics, never updated) and TRAIN_NO_PARAM_GRADS (input gradient only) only
 // change the BatchNorm arithmetic and which reductions run; the convolution-shaped passes are the same kernels. The same holds
 // per block (bn_frozen) and per parameter (null gradient slots), with an early stop below the lowest block that needs a
@@ -365,8 +367,21 @@ __global__ void train_bn_sync_bwd_finalize_kernel(const double *__restrict__ buf
     s2[c] = (float)(buf[C + c] / buf[2 * C]);
 }
 
-//   dz = invstd gamma (dy - mean(dy) - zh mean(dy zh))      written over ga (in place)
+//   dz = invstd gamma (dy - mean(dy) - zh mean(dy zh))      of element i of [B][C][L], from da = ga[i]
 // With s1 = s2 = 0 this is the eval-mode (frozen statistics) BatchNorm backward, dz = invstd gamma dy.
+__device__ __forceinline__ float bn_bwd_dz(const float *__restrict__ ga, const float *__restrict__ z, const float *__restrict__ mean,
+                                           const float *__restrict__ invstd, const float *__restrict__ gamma,
+                                           const float *__restrict__ beta, const float *__restrict__ s1,
+                                           const float *__restrict__ s2, long long i, int C, int L)
+{
+    const int c = (int)((i / L) % C);
+    const float zh = (z[i] - mean[c]) * invstd[c];
+    const float yv = fmaf(gamma[c], zh, beta[c]);
+    const float dyv = yv >= 0.f ? ga[i] : kLreluSlope * ga[i];
+    return invstd[c] * gamma[c] * (dyv - s1[c] - zh * s2[c]);
+}
+
+// dz written over ga (in place)
 __global__ void train_bn_bwd_apply_kernel(float *__restrict__ ga, const float *__restrict__ z, const float *__restrict__ mean,
                                           const float *__restrict__ invstd, const float *__restrict__ gamma,
                                           const float *__restrict__ beta, const float *__restrict__ s1,
@@ -374,11 +389,42 @@ __global__ void train_bn_bwd_apply_kernel(float *__restrict__ ga, const float *_
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long long)B * C * L) return;
-    const int c = (int)((i / L) % C);
-    const float zh = (z[i] - mean[c]) * invstd[c];
-    const float yv = fmaf(gamma[c], zh, beta[c]);
-    const float dyv = yv >= 0.f ? ga[i] : kLreluSlope * ga[i];
-    ga[i] = invstd[c] * gamma[c] * (dyv - s1[c] - zh * s2[c]);
+    ga[i] = bn_bwd_dz(ga, z, mean, invstd, gamma, beta, s1, s2, i, C, L);
+}
+
+// max |v| of a thread's values (as bits: non-negative floats order as their bits, NaN above inf) -> *amax, one atomicMax per
+// warp (*amax zeroed first); every lane of the warp calls it
+__device__ __forceinline__ void warp_amax_combine(unsigned m, float *amax)
+{
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(reinterpret_cast<unsigned *>(amax), m);
+}
+constexpr int kAmaxCtas = 8 * 132;         // grid of the max |dz| kernels (grid-stride): a few thousand atomics per block
+
+// TRAIN_FP16_SCALED: train_bn_bwd_apply_kernel's dz, and max |dz| of the block -> *amax (the block's scale slot)
+__global__ void __launch_bounds__(256) train_bn_bwd_apply_amax_kernel(float *__restrict__ ga, const float *__restrict__ z,
+                                                                      const float *__restrict__ mean, const float *__restrict__ invstd,
+                                                                      const float *__restrict__ gamma, const float *__restrict__ beta,
+                                                                      const float *__restrict__ s1, const float *__restrict__ s2,
+                                                                      int B, int C, int L, float *__restrict__ amax)
+{
+    const long long n = (long long)B * C * L;
+    unsigned m = 0;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const float d = bn_bwd_dz(ga, z, mean, invstd, gamma, beta, s1, s2, i, C, L);
+        ga[i] = d;
+        m = max(m, __float_as_uint(fabsf(d)));
+    }
+    warp_amax_combine(m, amax);
+}
+
+// max |src[i]| over n values -> *amax (zeroed first): the scale of dz in wunet_debug_train_conv
+__global__ void __launch_bounds__(256) train_amax_kernel(const float *__restrict__ src, long long n, float *__restrict__ amax)
+{
+    unsigned m = 0;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        m = max(m, __float_as_uint(fabsf(src[i])));
+    warp_amax_combine(m, amax);
 }
 
 // out[c] = sum over (b, l) of src[b][c][l]      (conv bias gradient: db = sum dz)
@@ -698,14 +744,15 @@ struct Layout {
     std::vector<size_t> z, act, ga;      // float offsets of the pre-BN outputs, activations, activation gradients
     std::vector<size_t> mean, invstd, s1, s2;
     std::vector<size_t> wf, wb;          // the step's packed weights: forward / input-gradient operand layouts
-    std::vector<size_t> wftc, wbtc;      // TRAIN_BF16 / TRAIN_TF32 only (appended after `total` of the fp32 layout): the
-                                         // tensor-core packings at that precision
+    std::vector<size_t> wftc, wbtc;      // the tensor-core precisions only (appended after the fp32 layout): the tensor-core
+                                         // packings at that precision
     size_t din, ones, zeros, total;      // ones / zeros: [kMaxC] identity scale and zero shift for the linear conv epilogue
+    size_t amax;                         // TRAIN_FP16_SCALED only (after the packings): [2n+1] max |dz| of each block (0 = none)
 };
 constexpr int kMaxC = 2048;
 
 // the first block (Cin = 1: a degenerate GEMM) stays on the fp32 kernels at every precision
-bool on_tc(int prec, int i) { return (prec == TRAIN_BF16 || prec == TRAIN_TF32) && i > 0; }
+bool on_tc(int prec, int i) { return (prec == TRAIN_BF16 || prec == TRAIN_TF32 || prec == TRAIN_FP16_SCALED) && i > 0; }
 
 // launch geometry of block i's weight gradient at `prec`
 WgradGrid wgrad_grid_of(int prec, int i, int B, int L, int cin, int cout, int k)
@@ -734,6 +781,7 @@ void layout_of(const std::vector<Shape> &sh, int B, Layout &lo, int prec = TRAIN
         lo.wftc[i] = take((train_tc_packed_bytes(prec, sh[i].cout, sh[i].cin, sh[i].k) + 3) / 4);       // float units
         lo.wbtc[i] = take((train_tc_packed_bytes(prec, sh[i].cin, sh[i].cout, sh[i].k) + 3) / 4);
     }
+    lo.amax = prec == TRAIN_FP16_SCALED ? take(nb) : 0;
     lo.total = cur;
 }
 
@@ -807,8 +855,9 @@ int train_debug_layout(int n, int ci, int B, int T, int prec, int block, long lo
         (long long)lo.z[block] * b, (long long)lo.act[block] * b, (long long)lo.ga[block] * b, (long long)lo.mean[block] * b,
         (long long)lo.invstd[block] * b, (long long)lo.s1[block] * b, (long long)lo.s2[block] * b,
         s.cin, s.cin0, s.cin1, s.cout, s.L, s.k, s.mode,
-        tc ? prec : 0 /* the field's 1 = bf16, 2 = tf32 are TRAIN_BF16, TRAIN_TF32 */, g.grid.x, g.grid.y, gz, g.items, g.positions, (g.items + gz - 1) / gz, (long long)lo.total * b};
+        tc ? prec : 0 /* the field's 1 = bf16, 2 = tf32, 3 = fp16 are TRAIN_BF16, TRAIN_TF32, TRAIN_FP16_SCALED */, g.grid.x, g.grid.y, gz, g.items, g.positions, (g.items + gz - 1) / gz, (long long)lo.total * b};
     for (int i = 0; i < kTrainLayoutFields; ++i) f[i] = v[i];
+    if (capacity > kTrainLayoutFields) f[kTrainLayoutFields] = (prec == TRAIN_FP16_SCALED && tc) ? (long long)(lo.amax + block) * b : -1;
     return 0;
 }
 
@@ -939,6 +988,8 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         }
     }
     const int i_hi = (part == 1) ? n : last, i_lo = std::max((part == 0) ? n + 1 : 0, j);
+    const bool scaled = prec == TRAIN_FP16_SCALED;
+    if (scaled && i_hi >= i_lo) cudaMemsetAsync(ws + lo.amax + i_lo, 0, (size_t)(i_hi - i_lo + 1) * sizeof(float), st);
     for (int i = i_hi; i >= i_lo; --i) {
         const Shape &s = sh[i];
         float *ga = ws + lo.ga[i];                               // gradient of the activation; becomes dz in place
@@ -958,9 +1009,15 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
             train_bn_bwd_stats_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
                                                                          g_gamma, g_beta, ws + lo.s1[i], ws + lo.s2[i], B, s.cout, s.L);
         const float *s1 = frozen ? ws + lo.zeros : ws + lo.s1[i], *s2 = frozen ? ws + lo.zeros : ws + lo.s2[i];
-        train_bn_bwd_apply_kernel<<<blocks_for(nel, 256), 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i],
-                                                                        s1, s2, B, s.cout, s.L);
-        const ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
+        // the scaled passes of this block read its max |dz| (wunet_train_tc_kernels.cuh)
+        float *amax = scaled && on_tc(prec, i) ? ws + lo.amax + i : nullptr;
+        if (amax)
+            train_bn_bwd_apply_amax_kernel<<<std::min(blocks_for(nel, 256), (unsigned)kAmaxCtas), 256, 0, st>>>(
+                ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i], P.bn_b[i], s1, s2, B, s.cout, s.L, amax);
+        else
+            train_bn_bwd_apply_kernel<<<blocks_for(nel, 256), 256, 0, st>>>(ga, z, ws + lo.mean[i], ws + lo.invstd[i], P.bn_w[i],
+                                                                            P.bn_b[i], s1, s2, B, s.cout, s.L);
+        ConvArgs a = conv_args(sh, lo, ws, x, i, n, B);
         if (g_cb) train_channel_sum_kernel<<<(unsigned)s.cout, 256, 0, st>>>(ga, g_cb, B, s.cout, s.L);
         if (g_cw) {
             // weight gradient: gridDim.z slices combined with atomicAdd into the zeroed dW or, in deterministic mode, stored to
@@ -970,6 +1027,7 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
             if (!det) cudaMemsetAsync(g_cw, 0, (size_t)nw * sizeof(float), st);
             const dim3 gw((unsigned)s.cout, (unsigned)((s.cin + 3) / 4), (unsigned)std::min(B, 8));
             if (on_tc(prec, i)) {
+                a.scale = amax;                                          // the weight gradient has no epilogue
                 if (launch_train_wgrad_tc(prec, a, ga, wdst, s.k, s.mode, st, det) < 0) return train_fail("training backward, block %d: tensor-core weight-gradient launch failed", i);
             } else if (!naive) {
                 launch_wgrad_fp32(a, ga, wdst, s.mode, st, det);
@@ -992,6 +1050,7 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
                 d.B = B; d.L = s.L; d.Cin = s.cout; d.Cin0 = s.cout; d.Cin1 = 0; d.Cout = s.cin; d.linear = 1;
                 if (on_tc(prec, i)) {
                     d.wp = ws + lo.wbtc[i];                                     // the packing the forward wrote
+                    d.src1 = amax;                                              // (DIRECT mode reads no skip input)
                     if (launch_train_conv_tc(prec, d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: tensor-core input-gradient launch failed", i);
                 } else if (launch_conv_fp32(d, s.k, SRC_DIRECT, st) < 0) return train_fail("training backward, block %d: input-gradient conv launch failed", i);
             } else if (s.k == 15) train_conv_bwd_data_kernel<15><<<gd, 128, 0, st>>>(ga, P.conv_w[i], din, B, s.cin, s.cout, s.L);
@@ -1026,7 +1085,7 @@ int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int 
 {
     const bool ok_mode = (ksize == 15 && (mode == SRC_DIRECT || mode == SRC_DECIM)) || (ksize == 5 && mode == SRC_UPCAT) ||
                          (ksize == 5 && mode == SRC_DIRECT && pass == 1);
-    if (pass < 0 || pass > 2 || (prec != TRAIN_FP32 && prec != TRAIN_BF16 && prec != TRAIN_TF32) || !ok_mode || B < 1 || L < 1 || Cin0 < 1 ||
+    if (pass < 0 || pass > 2 || (prec != TRAIN_FP32 && prec != TRAIN_BF16 && prec != TRAIN_TF32 && prec != TRAIN_FP16_SCALED) || !ok_mode || B < 1 || L < 1 || Cin0 < 1 ||
         Cin1 < 0 || Cout < 1 || (mode != SRC_UPCAT && Cin1 != 0) || (mode == SRC_UPCAT && (L < 2 || L % 2 != 0 || Cin1 < 1)) ||
         !w || !out || (pass != 1 && !src0) || (pass != 1 && mode == SRC_UPCAT && !src1) || (pass != 0 && !dz))
         return train_fail("debug conv: bad arguments");
@@ -1039,15 +1098,24 @@ int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int 
     const bool tc = prec != TRAIN_FP32;
     const size_t ntcf = tc ? train_tc_packed_bytes(prec, Cout, Cin, K) / sizeof(float) : 0;     // float units
     const size_t ntc = tc ? ntcf + train_tc_packed_bytes(prec, Cin, Cout, K) / sizeof(float) : 0;
-    if (cudaMalloc(&buf, (2 * cpad + 2 * wpad + ntc) * sizeof(float)) != cudaSuccess)
+    if (cudaMalloc(&buf, (2 * cpad + 2 * wpad + ntc + 64) * sizeof(float)) != cudaSuccess)
         return train_fail("debug conv: %s", cudaGetErrorString(cudaGetLastError()));
     float *ones = buf, *zeros = buf + cpad, *wf = zeros + cpad, *wb = wf + wpad, *wtc_f = wb + wpad, *wtc_b = wtc_f + ntcf;
     const cudaStream_t st = 0;
     train_fill_kernel<<<(cmax + 255) / 256, 256, 0, st>>>(ones, 1.f, cmax);
     train_fill_kernel<<<(cmax + 255) / 256, 256, 0, st>>>(zeros, 0.f, cmax);
+    // TRAIN_FP16_SCALED: the passes that read dz scale it by 2^k of its max |dz|, as the step does per block
+    float *amax = prec == TRAIN_FP16_SCALED && pass != 0 ? wtc_f + ntc : nullptr;
+    if (amax) {
+        const long long ndz = (long long)B * Cout * L;
+        cudaMemsetAsync(amax, 0, sizeof(float), st);
+        train_amax_kernel<<<std::min(blocks_for(ndz, 256), (unsigned)kAmaxCtas), 256, 0, st>>>(dz, ndz, amax);
+    }
+    if (mode != SRC_UPCAT) a.src1 = nullptr;                  // no skip input (and no scale: the forward conv is unscaled)
     int rc = 0;
     if (pass == 2) {
         cudaMemsetAsync(out, 0, nw * sizeof(float), st);
+        a.scale = amax;
         if (tc) rc = launch_train_wgrad_tc(prec, a, dz, out, K, mode, st, false);
         else launch_wgrad_fp32(a, dz, out, mode, st);
     } else {
@@ -1058,7 +1126,7 @@ int train_debug_conv(int pass, int prec, int mode, int ksize, int B, int L, int 
             if (rc >= 0) rc = tc ? launch_train_conv_tc(prec, a, K, mode, st) : launch_conv_fp32(a, K, mode, st);
         } else {
             ConvArgs d{};
-            d.src0 = dz; d.wp = tc ? wtc_b : wb; d.scale = ones; d.shift = zeros; d.out = out;
+            d.src0 = dz; d.src1 = amax; d.wp = tc ? wtc_b : wb; d.scale = ones; d.shift = zeros; d.out = out;
             d.B = B; d.L = L; d.Cin = Cout; d.Cin0 = Cout; d.Cin1 = 0; d.Cout = Cin; d.linear = 1;
             if (rc >= 0) rc = tc ? launch_train_conv_tc(prec, d, K, SRC_DIRECT, st) : launch_conv_fp32(d, K, SRC_DIRECT, st);
         }

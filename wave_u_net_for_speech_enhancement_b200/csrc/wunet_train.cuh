@@ -1,6 +1,7 @@
 // wunet_train.cuh — interface of the fp32 training step (implemented in wunet_train.cu; SURVEY.md §8f row N1).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stddef.h>
 
 namespace wunet {
@@ -26,8 +27,22 @@ struct TrainGrads {
 // dz; round to nearest), fp32 accumulation on the tensor cores (wunet_train_tc.cu); the first block stays fp32. Everything else
 // is fp32 at every precision. The workspace of TRAIN_BF16 is the fp32 one plus the bf16 weight packings. TRAIN_TF32: the same
 // with tf32 operands (round to nearest, ties away; the same kernels, templated on the operand type), its workspace the fp32
-// one plus the tf32 packings.
-enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1, TRAIN_TF32 = 2 };
+// one plus the tf32 packings. TRAIN_FP16_SCALED: fp16 operands (round to nearest even, overflow to inf), with each block's dz
+// scaled by 2^k (dz_scale_exp of its max |dz|, found on the device) for the two passes that read it and their results by 2^-k;
+// its workspace is the bf16 one with fp16 packings (the same bytes) plus 2n+1 scale slots (each block's max |dz|).
+enum TrainPrec : int { TRAIN_FP32 = 0, TRAIN_BF16 = 1, TRAIN_TF32 = 2, TRAIN_FP16_SCALED = 3 };
+
+// k of a block's dz scaling under TRAIN_FP16_SCALED, from amax = max |dz| over the block: amax 2^k lies in [2^13, 2^14), so the
+// scaled dz stays below a quarter of fp16's largest finite value (65504) and keeps 37 binades above its smallest subnormal;
+// k = 0 when amax is 0 or not finite (NaN, inf: those propagate unscaled); |k| <= 126, so 2^k and 2^-k are normal fp32 numbers.
+__host__ __device__ inline int dz_scale_exp(float amax)
+{
+    if (!(amax > 0.f && amax <= 3.402823466e38f)) return 0;
+    int e;
+    frexpf(amax, &e);                                           // amax = m 2^e, m in [0.5, 1): floor(log2 amax) = e - 1
+    const int k = 14 - e;
+    return k < -126 ? -126 : (k > 126 ? 126 : k);
+}
 // TRAIN_FROZEN_BN: BatchNorm normalises by the running statistics and never updates them (eval-mode BatchNorm); the forward
 // and the backward of one step must agree on it. TRAIN_NO_PARAM_GRADS (backward only): no parameter gradient is computed
 // (G may hold null pointers), only the input gradient. TRAIN_DETERMINISTIC: the weight and head gradients combine their

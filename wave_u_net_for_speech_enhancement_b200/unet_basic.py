@@ -310,7 +310,12 @@ class Model(nn.Module):
                    the operands rounded to tf32 (11 significant bits, round to nearest) instead, which is what cuDNN does
                    for Conv1d on an H100 under PyTorch's default ``torch.backends.cudnn.allow_tf32 = True``, i.e. the
                    reference's own training arithmetic there (that flag does not select it: the default stays "fp32").
-                   "bf16" and "tf32" only with train_backend="native". Not part of the state_dict.
+                   "fp16_scaled": the same with fp16 operands (round to nearest even) at bf16's speed, and each block's
+                   dz scaled inside the library by 2^k chosen on the device (max |dz| 2^k in [2^13, 2^14)), its results
+                   by 2^-k: exact, so no loss scaling is needed; non-finite values are not saturated and reach the
+                   gradients (a ``torch.amp.GradScaler`` then skips the step). Plain "fp16" (unscaled, autocast semantics)
+                   is not a training precision. "bf16", "tf32" and "fp16_scaled" only with train_backend="native". Not
+                   part of the state_dict.
     eval_autograd  when an eval-mode forward records an autograd graph (grad mode on, train_backend "native" or "torch").
                    "input" (default): when the input requires grad — ``x.grad`` of an upstream model or front end, input
                    gradients of an adversarial perturbation. "always": also when some parameter requires grad, for
@@ -509,7 +514,7 @@ class Model(nn.Module):
         its own container, as the reference's sub-modules do: in .train() it uses batch statistics and updates its running
         buffers with its own momentum (None: the cumulative factor 1 / num_batches_tracked) and counter; in .eval() it
         normalises by the running statistics and leaves them untouched. fp32 or, with ``train_precision="bf16"`` /
-        ``"tf32"``, bf16 / tf32 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
+        ``"tf32"`` / ``"fp16_scaled"``, bf16 / tf32 / fp16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
         self._check_input(x)
         B, _, T = x.shape
         blocks = self._blocks()
