@@ -51,6 +51,13 @@ extern "C" {
                                power-of-two scaling of dz, fp32 accumulate on wgmma tensor cores (see the training entry points);
                                the inference entry points reject it (WUNET_EINVAL) */
 
+/* element type of the network input x and output y (the _io entry points) */
+#define WUNET_IO_F32 0      /* float32 samples (what every entry point without _io takes) */
+#define WUNET_IO_F16 1      /* IEEE binary16 samples: widened to fp32 on load (exact); each output rounded once from the fp32
+                               result, to nearest even. Everything in between is the fp32-I/O computation at `precision`, so
+                               y = (fp16) forward(fp32(x)) bit for bit. */
+#define WUNET_IO_BF16 2     /* bfloat16 samples, the same contract */
+
 typedef struct wunet_ctx wunet_ctx;
 
 /* Version / build info string (static storage). */
@@ -93,7 +100,7 @@ size_t wunet_workspace_bytes(const wunet_ctx *ctx, int B, int T, int precision);
 
 /*
  * Replaces: Model.forward(input)   model/unet_basic.py:77-100   (eval-mode BatchNorm)
- *   x_dev [B,1,T] fp32 contiguous  ->  y_dev [B,1,T] fp32 contiguous, values in (-1,1).
+ *   x_dev [B,1,T] fp32 contiguous  ->  y_dev [B,1,T] fp32 contiguous, values in (-1,1) (16-bit: wunet_forward_io).
  * T must be a multiple of 2^n_layers (the reference raises from torch.cat at :95 otherwise)
  * -> WUNET_EINVAL.  Enqueues kernels on `stream` and returns; `workspace` must stay alive until
  * they finish.  Call sites this serves: trainer/trainer.py:75, enhancement.py:66.
@@ -103,6 +110,14 @@ size_t wunet_workspace_bytes(const wunet_ctx *ctx, int B, int T, int precision);
  */
 int wunet_forward(wunet_ctx *ctx, const float *x_dev, float *y_dev, int B, int T, int precision,
                   void *workspace, size_t workspace_bytes, void *stream);
+/*
+ * The same with x_dev / y_dev holding B*T samples of `io_dtype` (WUNET_IO_*): a half model's forward, 16-bit in and out. Only
+ * the first kernel's input read and the output write change (the kernels that touch x or y are instantiated per I/O type); the
+ * workspace is wunet_workspace_bytes()'s, whatever the I/O type. The parameters stay those of wunet_set_weights (fp32: a
+ * caller holding 16-bit parameters widens them, which is exact). wunet_forward() is io_dtype = WUNET_IO_F32.
+ */
+int wunet_forward_io(wunet_ctx *ctx, const void *x_dev, void *y_dev, int B, int T, int precision, int io_dtype,
+                     void *workspace, size_t workspace_bytes, void *stream);
 
 /*
  * Same operator with HOST buffers (the end-to-end form used by enhancement.py:64-66, which does
@@ -111,6 +126,8 @@ int wunet_forward(wunet_ctx *ctx, const float *x_dev, float *y_dev, int B, int T
  * x_host/y_host should be pinned for full PCIe rate; pageable memory also works.
  */
 int wunet_forward_host(wunet_ctx *ctx, const float *x_host, float *y_host, int B, int T, int precision);
+/* x_host / y_host of io_dtype (WUNET_IO_*): the copies move 2 bytes per sample for the 16-bit types */
+int wunet_forward_host_io(wunet_ctx *ctx, const void *x_host, void *y_host, int B, int T, int precision, int io_dtype);
 
 /*
  * Streaming form of the same operator for MANY batches — what enhancement.py:49-74 / trainer/trainer.py:58-79 do when they
@@ -121,6 +138,9 @@ int wunet_forward_host(wunet_ctx *ctx, const float *x_host, float *y_host, int B
  * the ticket has been waited for.
  */
 int wunet_stream_submit(wunet_ctx *ctx, const float *x_host, float *y_host, int B, int T, int precision, int *ticket);
+/* x_host / y_host of io_dtype (WUNET_IO_*); tickets are shared with wunet_stream_submit() */
+int wunet_stream_submit_io(wunet_ctx *ctx, const void *x_host, void *y_host, int B, int T, int precision, int io_dtype,
+                           int *ticket);
 int wunet_stream_wait(wunet_ctx *ctx, int ticket);
 
 /*
@@ -140,6 +160,12 @@ int wunet_frame_clips_i16(const int16_t *const *clips, const long long *lengths,
                           long long total_frames, int nthreads);
 int wunet_unframe_clips_f32(const float *frames, float *const *clips_out, const long long *lengths, int nclips, int sample_length,
                             long long total_frames, int nthreads);
+/* The two framing forms with frames of io_dtype (WUNET_IO_*), the staging buffer of wunet_stream_submit_io(): each sample is
+ * computed in fp32 as above (int16 PCM: sample / 32768) and rounded once to io_dtype (nearest even). */
+int wunet_frame_clips_f32_io(const float *const *clips, const long long *lengths, int nclips, int sample_length, void *frames,
+                             long long total_frames, int nthreads, int io_dtype);
+int wunet_frame_clips_i16_io(const int16_t *const *clips, const long long *lengths, int nclips, int sample_length, void *frames,
+                             long long total_frames, int nthreads, int io_dtype);
 
 /*
  * Training-side data path (SURVEY §8f row N4) - pure host code, no CUDA call. Replaces, per item of a batch, what

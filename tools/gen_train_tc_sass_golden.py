@@ -68,9 +68,9 @@ def keys_of(nvcc, names):
     return {n: kernel_key(d) for n, d in demangle(nvcc, names).items()}
 
 
-def kernels(nvcc, obj):
+def kernels(nvcc, obj, key_of=None):
     """{key: {"sass": sha256 of the normalised instruction lines, "res": resource line}} of every kernel in the object, plus the
-    normalised SASS itself under "lines" (not recorded in the golden)"""
+    normalised SASS itself under "lines" (not recorded in the golden). key_of: demangled name -> key (default: kernel_key)"""
     cuobjdump = os.path.join(os.path.dirname(nvcc), "cuobjdump")
     sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
     res = subprocess.run([cuobjdump, "-res-usage", obj], capture_output=True, text=True, check=True).stdout
@@ -78,7 +78,7 @@ def kernels(nvcc, obj):
     bodies = dict(zip(parts[1::2], parts[2::2]))
     usage = dict(re.findall(r"\n\s*Function (\S+):\n\s*(.+)", res))
     assert bodies.keys() == usage.keys(), (sorted(bodies), sorted(usage))
-    keys = keys_of(nvcc, list(bodies))
+    keys = keys_of(nvcc, list(bodies)) if key_of is None else {n: key_of(d) for n, d in demangle(nvcc, list(bodies)).items()}
     assert len(set(keys.values())) == len(keys), "two kernels share a key"
     out = {}
     for name, body in bodies.items():

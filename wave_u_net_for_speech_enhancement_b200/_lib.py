@@ -17,6 +17,10 @@ PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32_tc": PREC_FP32_TC, "fp
 TRAIN_PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32,      # training step (Model(train_precision=...))
                     "fp16_scaled": PREC_FP16_SCALED}
 
+IO_F32 = 0                 # element type of the network input / output (the _io entry points)
+IO_F16 = 1
+IO_BF16 = 2
+
 TRAIN_FROZEN_BN = 1        # training-step flags (include/wunet_b200.h): eval-mode BatchNorm
 TRAIN_NO_PARAM_GRADS = 2   # backward: input gradient only
 TRAIN_DETERMINISTIC = 16   # bitwise repeatable step (no float atomics; larger workspace)
@@ -56,11 +60,16 @@ def load() -> ctypes.CDLL:
     lib.wunet_forward_host.argtypes = [vp, vp, vp, ci, ci, ci]
     lib.wunet_stream_submit.argtypes = [vp, vp, vp, ci, ci, ci, ctypes.POINTER(ci)]
     lib.wunet_stream_wait.argtypes = [vp, ci]
+    lib.wunet_forward_io.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, cs, vp]
+    lib.wunet_forward_host_io.argtypes = [vp, vp, vp, ci, ci, ci, ci]
+    lib.wunet_stream_submit_io.argtypes = [vp, vp, vp, ci, ci, ci, ci, ctypes.POINTER(ci)]
     lib.wunet_read_level.argtypes = [vp, ci, vp, ci, ci, ci, vp, vp]
     ll = ctypes.c_longlong
     lib.wunet_frame_clips_f32.argtypes = [vp, vp, ci, ci, vp, ll, ci]
     lib.wunet_frame_clips_i16.argtypes = [vp, vp, ci, ci, vp, ll, ci]
     lib.wunet_unframe_clips_f32.argtypes = [vp, vp, vp, ci, ci, ll, ci]
+    lib.wunet_frame_clips_f32_io.argtypes = [vp, vp, ci, ci, vp, ll, ci, ci]
+    lib.wunet_frame_clips_i16_io.argtypes = [vp, vp, ci, ci, vp, ll, ci, ci]
     lib.wunet_wav_info.argtypes = [ctypes.c_char_p, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ll), ctypes.POINTER(ci), ctypes.POINTER(ci)]
     lib.wunet_wav_read_f32.argtypes = [ctypes.c_char_p, ll, ll, vp]
     lib.wunet_crop_pairs.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, ci]
@@ -109,6 +118,7 @@ EXPORTED_SYMBOLS = [
     "wunet_train_set_bn_allreduce", "wunet_train_forward_blocks", "wunet_train_backward_blocks", "wunet_debug_train_dz_scale",
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
+    "wunet_forward_io", "wunet_forward_host_io", "wunet_stream_submit_io", "wunet_frame_clips_f32_io", "wunet_frame_clips_i16_io",
 ]
 
 PLAN_FIELDS = ["L", "Cin0", "Cin1", "Cout", "Npad", "Nh", "nsplit", "Nstride", "MT", "nacc", "packed", "FR", "S", "m_tiles",

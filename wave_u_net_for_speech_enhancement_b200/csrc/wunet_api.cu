@@ -58,13 +58,13 @@ struct wunet_ctx {
     int ev_recorded = 0;
     // forward_host resources (grow-only)
     cudaStream_t hstream = nullptr;
-    float *hx = nullptr, *hy = nullptr;
+    void *hx = nullptr, *hy = nullptr;
     size_t hx_cap = 0;
     void *hws = nullptr;
     size_t hws_cap = 0;
     // streaming (double-buffered) host pipeline
     cudaStream_t s_in = nullptr, s_out = nullptr;
-    float *sx[2] = {nullptr, nullptr}, *sy[2] = {nullptr, nullptr};
+    void *sx[2] = {nullptr, nullptr}, *sy[2] = {nullptr, nullptr};
     size_t s_cap = 0;
     cudaEvent_t e_in[2] = {}, e_comp[2] = {}, e_done[2] = {};
     bool slot_busy[2] = {false, false};
@@ -120,7 +120,8 @@ cudaEvent_t *prof_events(wunet_ctx *c)
     return c->ev.data();
 }
 
-int forward_fp32(wunet_ctx *c, const float *x, float *y, int B, int T, void *ws, cudaStream_t st)
+// x, y: B*T samples of the IoType io; only block 0 (reads x) and the head (reads x, writes y) depend on it
+int forward_fp32(wunet_ctx *c, const void *x, void *y, int B, int T, void *ws, cudaStream_t st, int io)
 {
     const int n = c->n;
     std::vector<size_t> off;
@@ -134,14 +135,14 @@ int forward_fp32(wunet_ctx *c, const float *x, float *y, int B, int T, void *ws,
     for (int i = 0; i <= n; ++i) {                       // encoder (model/unet_basic.py:82-86) + middle (:88)
         const Block &bk = c->blocks[i];
         ConvArgs a{};
-        a.src0 = (i == 0) ? x : lvl(i - 1);
+        a.src0 = (i == 0) ? static_cast<const float *>(x) : lvl(i - 1);
         a.src1 = nullptr;
         a.wp = bk.wp; a.scale = bk.scale; a.shift = bk.shift;
         a.out = lvl(i);
         a.B = B; a.L = T >> i;
         a.Cin = bk.cin; a.Cin0 = bk.cin; a.Cin1 = 0; a.Cout = bk.cout;
         a.up_scale = 0.f;
-        const int r = launch_conv_fp32(a, bk.k, i == 0 ? SRC_DIRECT : SRC_DECIM, st);
+        const int r = (i == 0 && io != IO_F32) ? launch_conv_fp32_io(a, io, st) : launch_conv_fp32(a, bk.k, i == 0 ? SRC_DIRECT : SRC_DECIM, st);
         if (r < 0) return fail(WUNET_ECUDA, "encoder block %d launch failed: %s", i, cudaGetErrorString(cudaGetLastError()));
         launches += r;
         if (ev) cudaEventRecord(ev[i + 1], st);
@@ -165,7 +166,9 @@ int forward_fp32(wunet_ctx *c, const float *x, float *y, int B, int T, void *ws,
         if (ev) cudaEventRecord(ev[n + 2 + j], st);
     }
     {                                                    // out (model/unet_basic.py:98-99)
-        const int r = launch_out_fp32(lvl(2 * n), x, c->out_w, c->out_b, y, B, c->ci, T, st);
+        const int r = io == IO_F32 ? launch_out_fp32(lvl(2 * n), static_cast<const float *>(x), c->out_w, c->out_b, static_cast<float *>(y), B,
+                                                     c->ci, T, st)
+                                   : launch_out_fp32_io(lvl(2 * n), x, c->out_w, c->out_b, y, B, c->ci, T, io, st);
         if (r < 0) return fail(WUNET_ECUDA, "out launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         launches += r;
         if (ev) { cudaEventRecord(ev[2 * n + 2], st); c->ev_recorded = 2 * n + 3; }
@@ -306,11 +309,24 @@ size_t wunet_workspace_bytes(const wunet_ctx *c, int B, int T, int precision)
     return 0;
 }
 
+static int check_io(int io)
+{
+    if (io != WUNET_IO_F32 && io != WUNET_IO_F16 && io != WUNET_IO_BF16) return fail(WUNET_EINVAL, "unknown I/O dtype %d", io);
+    return WUNET_OK;
+}
+
 int wunet_forward(wunet_ctx *c, const float *x, float *y, int B, int T, int precision, void *workspace,
                   size_t workspace_bytes, void *stream)
 {
+    return wunet_forward_io(c, x, y, B, T, precision, WUNET_IO_F32, workspace, workspace_bytes, stream);
+}
+
+int wunet_forward_io(wunet_ctx *c, const void *x, void *y, int B, int T, int precision, int io, void *workspace,
+                     size_t workspace_bytes, void *stream)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
+    if (check_io(io) != WUNET_OK) return WUNET_EINVAL;
     if (!c->have_weights) return fail(WUNET_ESTATE, "wunet_forward called before wunet_set_weights");
     if (!x || !y || !workspace) return fail(WUNET_EINVAL, "null buffer");
     const size_t need = wunet_workspace_bytes(c, B, T, precision);
@@ -318,11 +334,11 @@ int wunet_forward(wunet_ctx *c, const float *x, float *y, int B, int T, int prec
     if (workspace_bytes < need) return fail(WUNET_ENOMEM, "workspace too small: %zu < %zu bytes", workspace_bytes, need);
     CUDA_TRY(cudaSetDevice(c->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (precision == WUNET_PREC_FP32) return forward_fp32(c, x, y, B, T, workspace, st);
+    if (precision == WUNET_PREC_FP32) return forward_fp32(c, x, y, B, T, workspace, st, io);
     int launches = 0;
     cudaEvent_t *ev = prof_events(c);
     if (tc_mode(precision) < 0) return fail(WUNET_EINVAL, "unknown precision %d", precision);
-    const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, tc_mode(precision));
+    const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, tc_mode(precision), io);
     if (ev && r == 0) c->ev_recorded = 2 * c->n + 3;
     if (r != 0) return fail(WUNET_ECUDA, "tensor-core forward failed: %s", tc_error());
     c->last_launches = launches;
@@ -331,12 +347,18 @@ int wunet_forward(wunet_ctx *c, const float *x, float *y, int B, int T, int prec
 
 int wunet_forward_host(wunet_ctx *c, const float *x_host, float *y_host, int B, int T, int precision)
 {
+    return wunet_forward_host_io(c, x_host, y_host, B, T, precision, WUNET_IO_F32);
+}
+
+int wunet_forward_host_io(wunet_ctx *c, const void *x_host, void *y_host, int B, int T, int precision, int io)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
+    if (check_io(io) != WUNET_OK) return WUNET_EINVAL;
     if (!x_host || !y_host) return fail(WUNET_EINVAL, "null host buffer");
     CUDA_TRY(cudaSetDevice(c->device));
     if (!c->hstream) CUDA_TRY(cudaStreamCreateWithFlags(&c->hstream, cudaStreamNonBlocking));
-    const size_t nbytes = (size_t)B * T * sizeof(float);
+    const size_t nbytes = (size_t)B * T * io_bytes(io);
     if (c->hx_cap < nbytes) {
         cudaFree(c->hx); cudaFree(c->hy);
         c->hx = c->hy = nullptr; c->hx_cap = 0;
@@ -356,13 +378,13 @@ int wunet_forward_host(wunet_ctx *c, const float *x_host, float *y_host, int B, 
         // chunked pipeline: H2D, first/last kernels and D2H overlap per batch chunk (see tc_forward_host)
         if (!c->have_weights) return fail(WUNET_ESTATE, "wunet_forward_host called before wunet_set_weights");
         int launches = 0;
-        if (tc_forward_host(c->tc, x_host, y_host, c->hx, c->hy, B, T, c->hws, c->hstream, &launches, tc_mode(precision)) != 0)
+        if (tc_forward_host(c->tc, x_host, y_host, c->hx, c->hy, B, T, c->hws, c->hstream, &launches, tc_mode(precision), io) != 0)
             return fail(WUNET_ECUDA, "tensor-core host pipeline failed: %s", tc_error());
         c->last_launches = launches;
         return WUNET_OK;
     }
     CUDA_TRY(cudaMemcpyAsync(c->hx, x_host, nbytes, cudaMemcpyHostToDevice, c->hstream));
-    rc = wunet_forward(c, c->hx, c->hy, B, T, precision, c->hws, c->hws_cap, c->hstream);
+    rc = wunet_forward_io(c, c->hx, c->hy, B, T, precision, io, c->hws, c->hws_cap, c->hstream);
     if (rc != WUNET_OK) return rc;
     CUDA_TRY(cudaMemcpyAsync(y_host, c->hy, nbytes, cudaMemcpyDeviceToHost, c->hstream));
     CUDA_TRY(cudaStreamSynchronize(c->hstream));
@@ -371,8 +393,14 @@ int wunet_forward_host(wunet_ctx *c, const float *x_host, float *y_host, int B, 
 
 int wunet_stream_submit(wunet_ctx *c, const float *x_host, float *y_host, int B, int T, int precision, int *ticket)
 {
+    return wunet_stream_submit_io(c, x_host, y_host, B, T, precision, WUNET_IO_F32, ticket);
+}
+
+int wunet_stream_submit_io(wunet_ctx *c, const void *x_host, void *y_host, int B, int T, int precision, int io, int *ticket)
+{
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
+    if (check_io(io) != WUNET_OK) return WUNET_EINVAL;
     if (!x_host || !y_host || !ticket) return fail(WUNET_EINVAL, "null argument");
     if (!c->have_weights) return fail(WUNET_ESTATE, "wunet_stream_submit called before wunet_set_weights");
     CUDA_TRY(cudaSetDevice(c->device));
@@ -386,7 +414,7 @@ int wunet_stream_submit(wunet_ctx *c, const float *x_host, float *y_host, int B,
             CUDA_TRY(cudaEventCreateWithFlags(&c->e_done[i], cudaEventDisableTiming));
         }
     }
-    const size_t nbytes = (size_t)B * T * sizeof(float);
+    const size_t nbytes = (size_t)B * T * io_bytes(io);
     const int k = c->next_ticket;
     const int slot = k & 1;
     if (c->slot_busy[slot]) { CUDA_TRY(cudaEventSynchronize(c->e_done[slot])); c->slot_busy[slot] = false; }
@@ -413,7 +441,7 @@ int wunet_stream_submit(wunet_ctx *c, const float *x_host, float *y_host, int B,
     CUDA_TRY(cudaMemcpyAsync(c->sx[slot], x_host, nbytes, cudaMemcpyHostToDevice, c->s_in));
     CUDA_TRY(cudaEventRecord(c->e_in[slot], c->s_in));
     CUDA_TRY(cudaStreamWaitEvent(c->hstream, c->e_in[slot], 0));
-    rc = wunet_forward(c, c->sx[slot], c->sy[slot], B, T, precision, c->hws, c->hws_cap, c->hstream);
+    rc = wunet_forward_io(c, c->sx[slot], c->sy[slot], B, T, precision, io, c->hws, c->hws_cap, c->hstream);
     if (rc != WUNET_OK) return rc;
     CUDA_TRY(cudaEventRecord(c->e_comp[slot], c->hstream));
     CUDA_TRY(cudaStreamWaitEvent(c->s_out, c->e_comp[slot], 0));
@@ -805,7 +833,12 @@ template <class Fn> void run_threads(long long nitems, int nthreads, Fn fn)
     for (auto &x : th) x.join();
 }
 
-template <class T> int frame_clips(FrameJob &j, float *frames, int nthreads)
+// O: element type of the frames (float, __half, __nv_bfloat16); each sample is computed in fp32 and rounded once to O
+template <class O> inline O frame_cvt(float v) { return v; }
+template <> inline __half frame_cvt<__half>(float v) { return __float2half_rn(v); }
+template <> inline __nv_bfloat16 frame_cvt<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+template <class T, class O = float> int frame_clips(FrameJob &j, O *frames, int nthreads)
 {
     if (!frames || j.SL <= 0 || j.nclips < 0 || j.total < 0 || (j.nclips > 0 && (!j.clips || !j.len))) return fail(WUNET_EINVAL, "frame_clips: bad argument");
     const int rc = build_job(j);
@@ -816,15 +849,16 @@ template <class T> int frame_clips(FrameJob &j, float *frames, int nthreads)
         const FrameJob &q = *jp;
         int ci = (int)(std::upper_bound(q.first.begin(), q.first.end(), f0) - q.first.begin()) - 1;   // clip holding frame f0
         for (long long f = f0; f < f1; ++f) {
-            float *dst = frames + f * q.SL;
-            if (f >= q.first[q.nclips]) { std::memset(dst, 0, sizeof(float) * q.SL); continue; }     // silent frames behind the clips
+            O *dst = frames + f * q.SL;
+            if (f >= q.first[q.nclips]) { std::memset(dst, 0, sizeof(O) * q.SL); continue; }         // silent frames behind the clips
             while (f >= q.first[ci + 1]) ++ci;
             const long long off = (f - q.first[ci]) * q.SL;
             const long long n = std::max<long long>(0, std::min<long long>(q.SL, q.len[ci] - off));
             const T *src = static_cast<const T *>(q.clips[ci]) + off;
-            if (sizeof(T) == sizeof(float)) std::memcpy(dst, src, sizeof(float) * n);
-            else for (long long k = 0; k < n; ++k) dst[k] = (float)src[k] * q.scale;
-            if (n < q.SL) std::memset(dst + n, 0, sizeof(float) * (q.SL - n));                        // enhancement.py:58 padding
+            if (sizeof(T) == sizeof(float) && sizeof(O) == sizeof(float)) std::memcpy(dst, src, sizeof(float) * n);
+            else if (sizeof(T) == sizeof(float)) for (long long k = 0; k < n; ++k) dst[k] = frame_cvt<O>((float)src[k]);
+            else for (long long k = 0; k < n; ++k) dst[k] = frame_cvt<O>((float)src[k] * q.scale);
+            if (n < q.SL) std::memset(dst + n, 0, sizeof(O) * (q.SL - n));                            // enhancement.py:58 padding
         }
     });
     return WUNET_OK;
@@ -846,6 +880,26 @@ int wunet_frame_clips_i16(const int16_t *const *clips, const long long *lengths,
 {
     FrameJob j{reinterpret_cast<const void *const *>(clips), lengths, nclips, sample_length, total_frames, 1.f / 32768.f, {}};
     return frame_clips<int16_t>(j, frames, nthreads);
+}
+
+int wunet_frame_clips_f32_io(const float *const *clips, const long long *lengths, int nclips, int sample_length, void *frames,
+                             long long total_frames, int nthreads, int io)
+{
+    if (check_io(io) != WUNET_OK) return WUNET_EINVAL;
+    FrameJob j{reinterpret_cast<const void *const *>(clips), lengths, nclips, sample_length, total_frames, 1.f, {}};
+    if (io == WUNET_IO_F16) return frame_clips<float>(j, static_cast<__half *>(frames), nthreads);
+    if (io == WUNET_IO_BF16) return frame_clips<float>(j, static_cast<__nv_bfloat16 *>(frames), nthreads);
+    return frame_clips<float>(j, static_cast<float *>(frames), nthreads);
+}
+
+int wunet_frame_clips_i16_io(const int16_t *const *clips, const long long *lengths, int nclips, int sample_length, void *frames,
+                             long long total_frames, int nthreads, int io)
+{
+    if (check_io(io) != WUNET_OK) return WUNET_EINVAL;
+    FrameJob j{reinterpret_cast<const void *const *>(clips), lengths, nclips, sample_length, total_frames, 1.f / 32768.f, {}};
+    if (io == WUNET_IO_F16) return frame_clips<int16_t>(j, static_cast<__half *>(frames), nthreads);
+    if (io == WUNET_IO_BF16) return frame_clips<int16_t>(j, static_cast<__nv_bfloat16 *>(frames), nthreads);
+    return frame_clips<int16_t>(j, static_cast<float *>(frames), nthreads);
 }
 
 int wunet_unframe_clips_f32(const float *frames, float *const *clips_out, const long long *lengths, int nclips, int sample_length,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stddef.h>
 
@@ -9,6 +10,48 @@ namespace wunet {
 
 constexpr float kBnEps = 1e-5f;       // torch.nn.BatchNorm1d default; reference model/unet_basic.py:12,25,55
 constexpr float kLreluSlope = 0.1f;   // reference model/unet_basic.py:13,26,56
+
+// Element type of the network input x and output y (WUNET_IO_* in include/wunet_b200.h). The kernels that read x or write y
+// take it as a template argument IO (float, __half or __nv_bfloat16): a sample is widened to fp32 on load (exact) and a result
+// rounded once to IO on store (round to nearest even); everything in between is the fp32-I/O computation.
+enum IoType : int { IO_F32 = 0, IO_F16 = 1, IO_BF16 = 2 };
+inline size_t io_bytes(int io) { return io == IO_F32 ? 4 : 2; }
+
+__device__ __forceinline__ float io_f32(float v) { return v; }
+__device__ __forceinline__ float io_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float io_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float io_ld(const float *p) { return __ldg(p); }
+__device__ __forceinline__ float io_ld(const __half *p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float io_ld(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
+__device__ __forceinline__ void io_st(float *p, float v) { *p = v; }
+__device__ __forceinline__ void io_st(__half *p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void io_st(__nv_bfloat16 *p, float v) { *p = __float2bfloat16_rn(v); }
+// four consecutive elements (16-byte aligned for float, 8-byte aligned for the 16-bit types)
+__device__ __forceinline__ float4 io_ld4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
+__device__ __forceinline__ float4 io_ld4(const __half *p)
+{
+    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(p));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2 *>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 io_ld4(const __nv_bfloat16 *p)
+{
+    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(p));
+    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&u.x));
+    const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ void io_st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
+__device__ __forceinline__ void io_st4(__half *p, float4 v)
+{
+    const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+    *reinterpret_cast<uint2 *>(p) = make_uint2(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b));
+}
+__device__ __forceinline__ void io_st4(__nv_bfloat16 *p, float4 v)
+{
+    const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+    *reinterpret_cast<uint2 *>(p) = make_uint2(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b));
+}
 
 // Where a conv block reads its input from (what the reference does between two Conv1d calls).
 enum SrcMode : int {
@@ -19,7 +62,7 @@ enum SrcMode : int {
 
 // One conv + eval-BN + LeakyReLU block on the fp32 path. All activations NCL fp32 (reference layout).
 struct ConvArgs {
-    const float *src0;   // DIRECT: [B][Cin][L]; DECIM: [B][Cin][2L]; UPCAT: prev [B][Cin0][L/2]
+    const float *src0;   // DIRECT: [B][Cin][L] (elements of the kernel's IO type: block 0 reads the network input); DECIM: [B][Cin][2L]; UPCAT: prev [B][Cin0][L/2]
     const float *src1;   // UPCAT: skip [B][Cin1][L]
     const float *wp;     // packed weights [Cin][K][Cout]  (Cout contiguous)
     const float *scale;  // [Cout]  gamma / sqrt(var + eps)
@@ -33,13 +76,13 @@ struct ConvArgs {
                          // conv output, input gradients)
 };
 
-// x -> NCL element fetch with zero padding outside [0, L)  (Conv1d padding, per frame)
-template <int MODE>
+// x -> NCL element fetch with zero padding outside [0, L)  (Conv1d padding, per frame); IO: element type of a DIRECT source
+template <int MODE, typename IO = float>
 __device__ __forceinline__ float fetch_src(const ConvArgs &a, int b, int ci, int l)
 {
     if (l < 0 || l >= a.L) return 0.f;
     if (MODE == SRC_DIRECT) {
-        return __ldg(a.src0 + ((size_t)b * a.Cin + ci) * a.L + l);
+        return io_ld(reinterpret_cast<const IO *>(a.src0) + ((size_t)b * a.Cin + ci) * a.L + l);
     } else if (MODE == SRC_DECIM) {
         return __ldg(a.src0 + ((size_t)b * a.Cin + ci) * (2 * (size_t)a.L) + 2 * l);
     } else {
@@ -70,6 +113,10 @@ __device__ __forceinline__ float bn_lrelu(float acc, float scale, float shift, i
 int launch_conv_fp32(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
 int launch_out_fp32(const float *dec, const float *x, const float *out_w, const float *out_b, float *y,
                     int B, int C, int T, cudaStream_t st);
+// block 0 (ksize 15, SRC_DIRECT) and the head with a 16-bit network input / output: a.src0, x and y hold IO elements (IoType io)
+int launch_conv_fp32_io(const ConvArgs &a, int io, cudaStream_t st);
+int launch_out_fp32_io(const float *dec, const void *x, const float *out_w, const float *out_b, void *y, int B, int C, int T,
+                       int io, cudaStream_t st);
 int launch_pack_fp32(const float *w, const float *bias, const float *g, const float *beta, const float *mean,
                      const float *var, float *wp, float *scale, float *shift, int Cout, int Cin, int K,
                      cudaStream_t st);

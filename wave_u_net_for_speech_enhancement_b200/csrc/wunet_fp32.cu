@@ -20,7 +20,7 @@ namespace wunet {
 // -------------------------------------------------------------------------------------------
 // sliding-window kernel
 // -------------------------------------------------------------------------------------------
-template <int KS, int MODE, int LW>
+template <int KS, int MODE, int LW, typename IO = float>
 __global__ void __launch_bounds__(96 * LW) conv_slide_kernel(const ConvArgs a)
 {
     constexpr int PAD = (KS - 1) / 2;
@@ -61,7 +61,7 @@ __global__ void __launch_bounds__(96 * LW) conv_slide_kernel(const ConvArgs a)
         __syncthreads();
         for (int i = tid; i < nci * XW; i += NT) {
             const int ci = i / XW, j = i - ci * XW;
-            Xs[ci][j] = fetch_src<MODE>(a, b, c0 + ci, l0 - PAD + j);
+            Xs[ci][j] = fetch_src<MODE, IO>(a, b, c0 + ci, l0 - PAD + j);
         }
         for (int i = tid; i < nci * KS * (COT / 4); i += NT) {
             const int row = i / (COT / 4), q = i - row * (COT / 4);      // row = ci*KS + k
@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(96 * LW) conv_slide_kernel(const ConvArgs a)
 // -------------------------------------------------------------------------------------------
 // generic implicit-GEMM kernel (im2col gather); positions p = b*L + l flattened over the batch
 // -------------------------------------------------------------------------------------------
-template <int KS, int MODE>
+template <int KS, int MODE, typename IO = float>
 __global__ void __launch_bounds__(128) conv_gen_kernel(const ConvArgs a)
 {
     constexpr int PAD = (KS - 1) / 2;
@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(128) conv_gen_kernel(const ConvArgs a)
         __syncthreads();
         for (int kk = (tid >> 6); kk < nk; kk += 2) {
             const int ci = kk / KS, k = kk - ci * KS;
-            Xs[kk][ln] = lvalid ? fetch_src<MODE>(a, lb, c0 + ci, ll + k - PAD) : 0.f;
+            Xs[kk][ln] = lvalid ? fetch_src<MODE, IO>(a, lb, c0 + ci, ll + k - PAD) : 0.f;
         }
         for (int i = tid; i < nk * BM; i += 128) {
             const int kk = i / BM, m = i - kk * BM;
@@ -186,11 +186,12 @@ __global__ void __launch_bounds__(128) conv_gen_kernel(const ConvArgs a)
 }
 
 // -------------------------------------------------------------------------------------------
-// out: cat([o, input], 1) -> Conv1d(C+1 -> 1, k=1) -> Tanh      (model/unet_basic.py:98-99, :72-75)
+// out: cat([o, input], 1) -> Conv1d(C+1 -> 1, k=1) -> Tanh      (model/unet_basic.py:98-99, :72-75); x, y: IO elements
 // -------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) out_kernel(const float *__restrict__ dec, const float *__restrict__ x,
+template <typename IO = float>
+__global__ void __launch_bounds__(256) out_kernel(const float *__restrict__ dec, const IO *__restrict__ x,
                                                   const float *__restrict__ w, const float *__restrict__ bias,
-                                                  float *__restrict__ y, int B, int C, int T)
+                                                  IO *__restrict__ y, int B, int C, int T)
 {
     const long long i4 = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 index over [B][T/4]
     const long long n4 = (long long)B * (T / 4);
@@ -206,10 +207,10 @@ __global__ void __launch_bounds__(256) out_kernel(const float *__restrict__ dec,
         acc.z = fmaf(wv, v.z, acc.z); acc.w = fmaf(wv, v.w, acc.w);
     }
     const float wx = __ldg(w + C);
-    const float4 xv = __ldg(reinterpret_cast<const float4 *>(x + (size_t)b * T + l));
+    const float4 xv = io_ld4(x + (size_t)b * T + l);
     acc.x = tanhf(fmaf(wx, xv.x, acc.x)); acc.y = tanhf(fmaf(wx, xv.y, acc.y));
     acc.z = tanhf(fmaf(wx, xv.z, acc.z)); acc.w = tanhf(fmaf(wx, xv.w, acc.w));
-    *reinterpret_cast<float4 *>(y + (size_t)b * T + l) = acc;
+    io_st4(y + (size_t)b * T + l, acc);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -240,19 +241,19 @@ __global__ void pack_fp32_kernel(const float *__restrict__ w, const float *__res
 // -------------------------------------------------------------------------------------------
 // launchers
 // -------------------------------------------------------------------------------------------
-template <int KS, int MODE>
+template <int KS, int MODE, typename IO = float>
 static int launch_conv_mode(const ConvArgs &a, cudaStream_t st)
 {
     if (a.L % 512 == 0 && a.Cout % 24 == 0) {
         dim3 grid(a.L / 512, a.Cout / 24, a.B);
-        conv_slide_kernel<KS, MODE, 2><<<grid, 192, 0, st>>>(a);
+        conv_slide_kernel<KS, MODE, 2, IO><<<grid, 192, 0, st>>>(a);
     } else if (a.L % 256 == 0 && a.Cout % 24 == 0) {
         dim3 grid(a.L / 256, a.Cout / 24, a.B);
-        conv_slide_kernel<KS, MODE, 1><<<grid, 96, 0, st>>>(a);
+        conv_slide_kernel<KS, MODE, 1, IO><<<grid, 96, 0, st>>>(a);
     } else {
         const long long P = (long long)a.B * a.L;
         dim3 grid((unsigned)((P + 63) / 64), (a.Cout + 47) / 48, 1);
-        conv_gen_kernel<KS, MODE><<<grid, 128, 0, st>>>(a);
+        conv_gen_kernel<KS, MODE, IO><<<grid, 128, 0, st>>>(a);
     }
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
@@ -288,6 +289,27 @@ int launch_out_fp32(const float *dec, const float *x, const float *out_w, const 
 {
     const long long n4 = (long long)B * (T / 4);
     out_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(dec, x, out_w, out_b, y, B, C, T);
+    return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_conv_fp32_io(const ConvArgs &a, int io, cudaStream_t st)
+{
+    if (io == IO_F16) return launch_conv_mode<15, SRC_DIRECT, __half>(a, st);
+    if (io == IO_BF16) return launch_conv_mode<15, SRC_DIRECT, __nv_bfloat16>(a, st);
+    return launch_conv_fp32(a, 15, SRC_DIRECT, st);
+}
+
+int launch_out_fp32_io(const float *dec, const void *x, const float *out_w, const float *out_b, void *y, int B, int C, int T,
+                       int io, cudaStream_t st)
+{
+    const long long n4 = (long long)B * (T / 4);
+    const unsigned grid = (unsigned)((n4 + 255) / 256);
+    if (io == IO_F16)
+        out_kernel<<<grid, 256, 0, st>>>(dec, static_cast<const __half *>(x), out_w, out_b, static_cast<__half *>(y), B, C, T);
+    else if (io == IO_BF16)
+        out_kernel<<<grid, 256, 0, st>>>(dec, static_cast<const __nv_bfloat16 *>(x), out_w, out_b, static_cast<__nv_bfloat16 *>(y), B, C, T);
+    else
+        return launch_out_fp32(dec, static_cast<const float *>(x), out_w, out_b, static_cast<float *>(y), B, C, T, st);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -1000,17 +1000,23 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
     return 0;
 }
 
-static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const float *x = nullptr, float *y = nullptr);
+static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const void *x = nullptr, void *y = nullptr,
+                        int io = IO_F32);
 
-// enc0 over frames [f0, f0 + nf); *launches receives the number of kernels enqueued
-static int launch_enc0(TcState *st, const float *x, int f0, int nf, int T, void *ws, cudaStream_t stream, int *launches = nullptr)
+// enc0 over frames [f0, f0 + nf) of x (IoType io samples: the 16-bit forms are those of wunet_tc_io.cuh); *launches receives the
+// number of kernels enqueued
+static int launch_enc0(TcState *st, const void *x_io, int f0, int nf, int T, void *ws, cudaStream_t stream, int *launches, int io)
 {
     if (launches) *launches = 1;
+    const void *xf = static_cast<const char *>(x_io) + (size_t)f0 * T * io_bytes(io);     // the frames' first sample
+    const float *x = static_cast<const float *>(xf);                                      // io == IO_F32
     if (st->plan.enc0_tc) {
         // tensor-core form: bf16 copy of the frames' samples, then block 0 as a 3-tap block over groups of 8 samples
         __nv_bfloat16 *xb = reinterpret_cast<__nv_bfloat16 *>(static_cast<char *>(ws) + st->plan.off[2 * st->n + 2]) + (size_t)f0 * T;
         const long long n4 = (long long)nf * T / 4;
-        x_to_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(x + (size_t)f0 * T, xb, n4);
+        if (io == IO_F16) io_f16::launch_x_to_bf16(xf, xb, n4, stream);
+        else if (io == IO_BF16) io_bf16::launch_x_to_bf16(xf, xb, n4, stream);
+        else x_to_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(x, xb, n4);
         if (cudaGetLastError() != cudaSuccess) return tc_fail("x_to_bf16_kernel launch failed");
         const int tpf = st->plan.lv[0].p.tiles_per_frame * st->plan.lv[0].p.nsplit;    // tiles of one frame, all column splits
         if (launches) *launches = 2;
@@ -1032,26 +1038,31 @@ static int launch_enc0(TcState *st, const float *x, int f0, int nf, int T, void 
     __nv_bfloat16 *even = (st->plan.even_copy && !split)
                               ? reinterpret_cast<__nv_bfloat16 *>(static_cast<char *>(ws) + st->plan.off[2 * st->n + 1]) + (size_t)f0 * (T / 2) * C
                               : nullptr;
-    const bool persistent = st->enc0_v == 2 || (st->enc0_v == 0 && split);
+    // the persistent form streams float samples (4-byte cp.async): a 16-bit input takes the one-tile form and its grid
+    const bool persistent = io == IO_F32 && (st->enc0_v == 2 || (st->enc0_v == 0 && split));
     if (persistent) {
         const int total = nf * ((T + 1023) / 1024);
         cfg.gridDim = dim3((unsigned)std::min(total, st->num_sms * 4), 1, 1);
     }
     if (st->ci > 32)                                    // wide plans: a tile that shrinks with C (no even-row copy: no row-pair form)
-        wide::launch_enc0(cfg, st->plan_mode, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C);
+        wide::launch_enc0(cfg, st->plan_mode, xf, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, io);
+    else if (io == IO_F16)
+        io_f16::launch_enc0(cfg, st->plan_mode, xf, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, even);
+    else if (io == IO_BF16)
+        io_bf16::launch_enc0(cfg, st->plan_mode, xf, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, even);
     else if (st->plan_mode == 2)                        // fp16: the same kernels with fp16 rows (same size as bf16 ones)
-        f16::launch_enc0(cfg, persistent, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, even);
+        f16::launch_enc0(cfg, persistent, x, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, even);
     else if (persistent)
-        cudaLaunchKernelEx(&cfg, enc0_kernel_v2, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, split, even);
+        cudaLaunchKernelEx(&cfg, enc0_kernel_v2, x, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, split, even);
     else
-        cudaLaunchKernelEx(&cfg, enc0_kernel, x + (size_t)f0 * T, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, split, even);
+        cudaLaunchKernelEx(&cfg, enc0_kernel, x, lv.w_src, lv.scale, lv.shift, out0 + (size_t)f0 * T * RC, nf, T, C, split, even);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return tc_fail("enc0 launch failed: %s", cudaGetErrorString(e));
     return 0;
 }
 
 // conv block i over the tile range [t0, t1) (t1 < 0: all tiles)
-static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const float *x, float *y)
+static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const void *x, void *y, int io)
 {
     TcPlanLevel &P = st->plan.lv[i];
     if (P.is_gemm) {
@@ -1067,7 +1078,7 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
         return 0;
     }
     TcParams p = P.p;
-    p.x = x; p.y = y;                                    // only the fused head (last block) reads x / writes y
+    p.x = static_cast<const float *>(x); p.y = static_cast<float *>(y);   // only the fused head (last block) reads x / writes y (IO samples)
     p.pf_late = st->pf_late ? 1 : 0;
     if (t1 >= 0) { p.tile_begin = t0; p.tile_end = t1; }
     const int ntiles = p.tile_end - p.tile_begin;
@@ -1078,7 +1089,13 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = st->pdl ? 1 : 0;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    if (st->plan_mode == 2) {
+    if (io != IO_F32 && p.head) {
+        // 16-bit network input / output: the last block's forms of wunet_tc_io.cuh (large flavour; not the row-pair form)
+        if (P.small || P.pair || !P.upcat || p.split == 2) return tc_fail("the last block's tiling has no 16-bit I/O form (small flavour)");
+        const int mode = st->plan_mode == 2 ? 2 : (p.split ? 1 : 0);
+        cudaLaunchKernelEx(&cfg, io == IO_F16 ? io_f16::head_kernel(mode, p.mg != 0) : io_bf16::head_kernel(mode, p.mg != 0), P.tmA, P.tmW,
+                           P.tmO, p);
+    } else if (st->plan_mode == 2) {
         // fp16: the twins of the bf16 forms below (no split-precision form, no block 0 over groups of 8)
         cudaLaunchKernelEx(&cfg, f16::conv_kernel(P.pair == 1 ? 9 : (P.upcat ? 5 : 15), P.small, P.upcat && p.mg), P.tmA, P.tmW, P.tmO, p);
     } else if (P.pair == 3) {
@@ -1107,19 +1124,19 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
     return 0;
 }
 
-int tc_forward(TcState *st, const float *x, float *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
-               cudaEvent_t *ev, int mode)
+int tc_forward(TcState *st, const void *x, void *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
+               cudaEvent_t *ev, int mode, int io)
 {
-    if (tc_prepare(st, x, y, B, T, ws, mode, stream)) return -1;
+    if (tc_prepare(st, nullptr, nullptr, B, T, ws, mode, stream)) return -1;
     const int n = st->n;
     int nl = 0;
     if (ev) cudaEventRecord(ev[0], stream);
     int l0n = 1;
-    if (launch_enc0(st, x, 0, B, T, ws, stream, &l0n)) return -1;
+    if (launch_enc0(st, x, 0, B, T, ws, stream, &l0n, io)) return -1;
     nl += l0n;
     if (ev) cudaEventRecord(ev[1], stream);
     for (int i = 1; i < 2 * n + 1; ++i) {
-        if (launch_block(st, i, 0, -1, stream, x, y)) return -1;
+        if (launch_block(st, i, 0, -1, stream, x, y, io)) return -1;
         ++nl;
         if (ev) cudaEventRecord(ev[i + 1], stream);
     }
@@ -1130,10 +1147,10 @@ int tc_forward(TcState *st, const float *x, float *y, int B, int T, void *ws, cu
 
 // Host-buffer pipeline (enhancement.py:64-66 form): the first kernel (enc0) and the last (decoder + fused head) run per
 // batch chunk, so the H2D copy of chunk c+1 overlaps enc0 of chunk c and the D2H copy of chunk c overlaps the head of c+1.
-int tc_forward_host(TcState *st, const float *x_host, float *y_host, float *x_dev, float *y_dev, int B, int T, void *ws,
-                    cudaStream_t stream, int *launches, int mode)
+int tc_forward_host(TcState *st, const void *x_host, void *y_host, void *x_dev, void *y_dev, int B, int T, void *ws,
+                    cudaStream_t stream, int *launches, int mode, int io)
 {
-    if (tc_prepare(st, x_dev, y_dev, B, T, ws, mode, stream)) return -1;
+    if (tc_prepare(st, nullptr, nullptr, B, T, ws, mode, stream)) return -1;
     const int n = st->n;
     const TcParams &pl = st->plan.lv[2 * n].p;
     int nc = 1;
@@ -1148,17 +1165,19 @@ int tc_forward_host(TcState *st, const float *x_host, float *y_host, float *x_de
         }
     }
     const int bc = B / nc;
-    const size_t chunk = (size_t)bc * T;
+    const size_t chunk = (size_t)bc * T * io_bytes(io);           // bytes of one chunk's samples
+    const char *xh = static_cast<const char *>(x_host);
+    char *yh = static_cast<char *>(y_host), *xd = static_cast<char *>(x_dev), *yd = static_cast<char *>(y_dev);
     int nl = 0;
     // the compute stream may still own x_dev/y_dev from an earlier call: order the copies after it
     cudaEventRecord(st->ev_out[7], stream);
     cudaStreamWaitEvent(st->copy_in, st->ev_out[7], 0);
     for (int c = 0; c < nc; ++c) {
-        cudaMemcpyAsync(x_dev + c * chunk, x_host + c * chunk, chunk * sizeof(float), cudaMemcpyHostToDevice, st->copy_in);
+        cudaMemcpyAsync(xd + c * chunk, xh + c * chunk, chunk, cudaMemcpyHostToDevice, st->copy_in);
         cudaEventRecord(st->ev_in[c], st->copy_in);
         cudaStreamWaitEvent(stream, st->ev_in[c], 0);
         int l0n = 1;
-        if (launch_enc0(st, x_dev, c * bc, bc, T, ws, stream, &l0n)) return -1;
+        if (launch_enc0(st, x_dev, c * bc, bc, T, ws, stream, &l0n, io)) return -1;
         nl += l0n;
     }
     for (int i = 1; i < 2 * n; ++i) {
@@ -1167,12 +1186,12 @@ int tc_forward_host(TcState *st, const float *x_host, float *y_host, float *x_de
     }
     const int tiles_per_chunk = (pl.m_tiles * pl.nsplit) / nc;      // non-packed: m_tiles = B * tiles_per_frame
     for (int c = 0; c < nc; ++c) {
-        if (nc == 1) { if (launch_block(st, 2 * n, 0, -1, stream, x_dev, y_dev)) return -1; }
-        else if (launch_block(st, 2 * n, c * tiles_per_chunk, (c + 1) * tiles_per_chunk, stream, x_dev, y_dev)) return -1;
+        if (nc == 1) { if (launch_block(st, 2 * n, 0, -1, stream, x_dev, y_dev, io)) return -1; }
+        else if (launch_block(st, 2 * n, c * tiles_per_chunk, (c + 1) * tiles_per_chunk, stream, x_dev, y_dev, io)) return -1;
         ++nl;
         cudaEventRecord(st->ev_out[c], stream);
         cudaStreamWaitEvent(st->copy_out, st->ev_out[c], 0);
-        cudaMemcpyAsync(y_host + c * chunk, y_dev + c * chunk, chunk * sizeof(float), cudaMemcpyDeviceToHost, st->copy_out);
+        cudaMemcpyAsync(yh + c * chunk, yd + c * chunk, chunk, cudaMemcpyDeviceToHost, st->copy_out);
     }
     if (cudaStreamSynchronize(st->copy_out) != cudaSuccess) return tc_fail("host pipeline failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (launches) *launches = nl;

@@ -23,11 +23,12 @@ int tc_set_weights(TcState **st, int n_layers, int ci, const TcBlockSrc *blocks,
 // 2 = fp16 activations and weights (the bf16 layout and plan; the fp16 weights are packed by the first fp16 forward)
 size_t tc_workspace_bytes(int n_layers, int ci, int B, int T, int mode = 0);
 // events: null, or 2n+3 events: [0] before the first kernel, [i+1] after block i, [2n+2] after the head
-int tc_forward(TcState *st, const float *x, float *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
-               cudaEvent_t *events, int mode = 0);
-// host-buffer form: x_host/y_host (pinned for full rate), x_dev/y_dev = device staging buffers of B*T floats
-int tc_forward_host(TcState *st, const float *x_host, float *y_host, float *x_dev, float *y_dev, int B, int T, void *ws,
-                    cudaStream_t stream, int *launches, int mode = 0);
+// x, y: B*T samples of the IoType io (wunet_common.cuh)
+int tc_forward(TcState *st, const void *x, void *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
+               cudaEvent_t *events, int mode = 0, int io = 0);
+// host-buffer form: x_host/y_host (pinned for full rate), x_dev/y_dev = device staging buffers of B*T samples of the IoType io
+int tc_forward_host(TcState *st, const void *x_host, void *y_host, void *x_dev, void *y_dev, int B, int T, void *ws,
+                    cudaStream_t stream, int *launches, int mode = 0, int io = 0);
 int tc_read_level(TcState *st, int block, const void *ws, int B, int T, float *out_ncl, cudaStream_t stream, int mode = 0);
 void tc_destroy(TcState *st);
 // host-only: the tiling build_plan would choose for `block` (32 ints, see wunet_debug_plan in include/wunet_b200.h); mode 1 =

@@ -216,12 +216,31 @@ namespace wide {
 using ConvKernel = f16::ConvKernel;
 void set_smem_attributes();
 // block 0 with a tile that shrinks with C; mode 0 = bf16, 1 = split precision, 2 = fp16. Sets cfg's grid, block and shared memory.
-cudaError_t launch_enc0(cudaLaunchConfig_t cfg, int mode, const float *x, const float *w, const float *scale, const float *shift, void *out,
-                        int B, int T, int C);
+// x: B*T samples of the IoType io (16-bit: the io_f16 / io_bf16 form, on the same grid)
+cudaError_t launch_enc0(cudaLaunchConfig_t cfg, int mode, const void *x, const float *w, const float *scale, const float *shift, void *out,
+                        int B, int T, int C, int io);
 // split-precision conv form for blocks of more than 48 K-loop positions (chunk_map lists chunks: chunk_info, SP = 2); large flavour
 ConvKernel conv_split_kernel(bool upcat);
 // its weights: tab lists the chunks (base, width) and the positions (n = 3 x chunks)
 cudaError_t pack_split(const float *w, void *wp, int Cout, int Cin, int K, int Npad, const SplitTable &tab, cudaStream_t stream);
 }  // namespace wide
+
+// The forms with a 16-bit network input / output (wunet_tc_io.cuh): io_f16 (__half, wunet_tc_io_f16.cu) and io_bf16
+// (__nv_bfloat16, wunet_tc_io_bf16.cu) have the same functions. mode: 0 = bf16, 1 = split precision, 2 = fp16 (tc_* modes).
+#define WUNET_TC_IO_DECLS                                                                                                           \
+    /* the last block (fused head), large flavour; mg: its K loop ends in a merged tail chunk (bf16 / fp16 modes) */                  \
+    ::wunet::f16::ConvKernel head_kernel(int mode, bool mg);                                                                                 \
+    void set_smem_attributes(int enc0_wide_max);                                                                                    \
+    /* block 0, one tile per CTA (enc0_kernel's grid and shared memory in cfg) */                                                   \
+    cudaError_t launch_enc0(const cudaLaunchConfig_t &cfg, int mode, const void *x, const float *w, const float *scale,             \
+                            const float *shift, void *out, int B, int T, int C, void *even_out);                                   \
+    /* block 0 of the wide plans (enc0_wide_kernel's grid and shared memory in cfg) */                                              \
+    cudaError_t launch_enc0_wide(const cudaLaunchConfig_t &cfg, int mode, const void *x, const float *w, const float *scale,        \
+                                 const float *shift, void *out, int B, int T, int C);                                              \
+    /* the bf16 copy of the input for the group-of-8 block 0 */                                                                     \
+    cudaError_t launch_x_to_bf16(const void *x, __nv_bfloat16 *xb, long long n4, cudaStream_t stream);
+namespace io_f16 { WUNET_TC_IO_DECLS }
+namespace io_bf16 { WUNET_TC_IO_DECLS }
+#undef WUNET_TC_IO_DECLS
 
 }  // namespace wunet

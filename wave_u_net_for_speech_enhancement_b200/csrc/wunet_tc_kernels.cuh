@@ -8,6 +8,13 @@
 
 using TcT = TcElem::T;            // activation / weight element
 using TcT2 = TcElem::T2;          // two of them (packed HFMA2 arithmetic)
+// Element type of the network input read by block 0 and the fused head, and of the output the head writes (IoType): float,
+// unless the includer defines WUNET_TC_IO as a 16-bit type (wunet_tc_io.cuh). A sample is widened to fp32 on load and a
+// result rounded once on store, so the float forms are the code they were before the I/O type existed.
+#ifndef WUNET_TC_IO
+#define WUNET_TC_IO float
+#endif
+using TcIO = WUNET_TC_IO;
 
 namespace {
 
@@ -484,8 +491,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         hsum += __shfl_xor_sync(0xffffffffu, hsum, 1);
                         hsum += __shfl_xor_sync(0xffffffffu, hsum, 2);
                         if (valid && (lane & 3) == 0) {
-                            const float hacc = fmaf(hw[p.Cout], __ldg(p.x + (size_t)bb * p.T + l), hw[p.Cout + 1] + hsum);
-                            p.y[(size_t)bb * p.T + l] = tanh_fast(hacc);
+                            const float hacc = fmaf(hw[p.Cout], io_ld(reinterpret_cast<const TcIO *>(p.x) + (size_t)bb * p.T + l),
+                                                    hw[p.Cout + 1] + hsum);
+                            io_st(reinterpret_cast<TcIO *>(p.y) + (size_t)bb * p.T + l, tanh_fast(hacc));
                         }
                     }
                 }
@@ -957,7 +965,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
 // WUNET_TC_CONV_ONLY (wunet_tc_wide.cu): the includer instantiates conv_tc_kernel forms of its own and needs none of the
 // non-template kernels below, which the other two units already emit.
+// WUNET_TC_IO_ONLY (wunet_tc_io.cuh): the forms with a 16-bit network input / output, i.e. conv_tc_kernel (instantiated by the
+// includer for the last block), enc0_kernel and x_to_bf16_kernel; none of the other kernels.
 #ifndef WUNET_TC_CONV_ONLY
+#ifndef WUNET_TC_IO_ONLY
 // -------------------------------------------------------------------------------------------------
 // bottom of the U (frames of at most 16 samples): the block as ONE dense GEMM over frames
 // -------------------------------------------------------------------------------------------------
@@ -1115,10 +1126,12 @@ __global__ void expand_gemm_weights_kernel(const float *__restrict__ w, TcT *__r
     wx[i] = TcElem::cvt(v);
 }
 
+#endif  // WUNET_TC_IO_ONLY
+
 // -------------------------------------------------------------------------------------------------
-// enc0: Conv1d(1 -> C, k=15) + BN + LeakyReLU on CUDA cores (Cin = 1: K = 15, HBM-bound), fp32 in, 16-bit NLC out
+// enc0: Conv1d(1 -> C, k=15) + BN + LeakyReLU on CUDA cores (Cin = 1: K = 15, HBM-bound), IO in (widened to fp32), 16-bit NLC out
 // -------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256, 4) enc0_kernel(const float *__restrict__ x, const float *__restrict__ w /*[C][1][15]*/,
+__global__ void __launch_bounds__(256, 4) enc0_kernel(const TcIO *__restrict__ x, const float *__restrict__ w /*[C][1][15]*/,
                                                       const float *__restrict__ scale, const float *__restrict__ shift,
                                                       TcT *__restrict__ out, int B, int T, int C, int split,
                                                       TcT *__restrict__ even_out)
@@ -1144,7 +1157,7 @@ __global__ void __launch_bounds__(256, 4) enc0_kernel(const float *__restrict__ 
     asm volatile("griddepcontrol.wait;" ::: "memory");
     for (int i = threadIdx.x; i < TILE + 16; i += 256) {
         const int l = l0 - PAD + i - 1;                       // xs[i] = x[l0 - 8 + i] so that a thread's window starts 16-byte aligned
-        xs[i] = (l >= 0 && l < T) ? x[(size_t)b * T + l] : 0.f;
+        xs[i] = (l >= 0 && l < T) ? io_f32(x[(size_t)b * T + l]) : 0.f;
     }
     __syncthreads();
     // window: positions 4*tid .. 4*tid+3 need x[l-7 .. l+3+7] = xs[4*tid + 1 .. 4*tid + 18]; load xs[4*tid .. 4*tid+19]
@@ -1201,10 +1214,12 @@ __global__ void __launch_bounds__(256, 4) enc0_kernel(const float *__restrict__ 
     }
 }
 
+#ifndef WUNET_TC_IO_ONLY
 // enc0, persistent form (round 2, last session): the same arithmetic in the same order (bit-identical output), but a block loops over
 // tiles: the weights are loaded once, the samples of the NEXT tile stream into shared memory by cp.async while this tile is
 // computed, and the bulk store of a tile's rows drains while the next tile's first channel pass is computed (the one-shot
 // kernel above spends ~35 % of its time in the un-overlapped load -> compute -> store -> drain phases of its 4 resident blocks).
+// float input only: a 16-bit input runs enc0_kernel (same output), since no cp.async form widens 16-bit samples
 __global__ void __launch_bounds__(256, 4) enc0_kernel_v2(const float *__restrict__ x, const float *__restrict__ w /*[C][1][15]*/,
                                                          const float *__restrict__ scale, const float *__restrict__ shift,
                                                          TcT *__restrict__ out, int B, int T, int C, int split,
@@ -1301,7 +1316,10 @@ __global__ void __launch_bounds__(256, 4) enc0_kernel_v2(const float *__restrict
     if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
+#endif  // WUNET_TC_IO_ONLY
+
 #ifndef WUNET_TC_FP16
+#ifndef WUNET_TC_IO_ONLY
 // -------------------------------------------------------------------------------------------------
 // row-pair mode: a K-tap conv block over positions as a K'-tap block over PAIRS of positions
 // -------------------------------------------------------------------------------------------------
@@ -1352,16 +1370,18 @@ __global__ void expand_group8_weights_kernel(const float *__restrict__ w, const 
     }
     if (i < 8 * Cout) { scale_v[i] = scale[i % Cout]; shift_v[i] = shift[i % Cout]; }
 }
-__global__ void x_to_bf16_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ xb, long long n4)
+#endif  // WUNET_TC_IO_ONLY
+__global__ void x_to_bf16_kernel(const TcIO *__restrict__ x, __nv_bfloat16 *__restrict__ xb, long long n4)
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n4) return;
-    const float4 v = __ldg(reinterpret_cast<const float4 *>(x) + i);
+    const float4 v = io_ld4(x + 4 * i);
     reinterpret_cast<uint2 *>(xb)[i] = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
 }
 
 #endif
 
+#ifndef WUNET_TC_IO_ONLY
 // weights [Cout][Cin][K] fp32 -> [K][Npad][Ktot] 16-bit elements, K axis = [seg0 padded to 64 | seg1 padded to 64], zero padded
 __global__ void pack_tc_kernel(const float *__restrict__ w, const float *__restrict__ scale, const float *__restrict__ shift,
                                TcT *__restrict__ wp, float2 *__restrict__ ss, int Cout, int Cin0, int Cin1, int K,
@@ -1458,4 +1478,5 @@ __global__ void nlc_f16_to_ncl_f32_kernel(const __half *__restrict__ src, float 
     dst[i] = TcElem::to_f32(src[((size_t)b * L + l) * C + c]);
 }
 
+#endif  // WUNET_TC_IO_ONLY
 #endif  // WUNET_TC_CONV_ONLY

@@ -52,16 +52,21 @@ void set_smem_attributes()
     cudaFuncSetAttribute(bf16::enc0_wide_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, enc0_max);
     cudaFuncSetAttribute(bf16::enc0_wide_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, enc0_max);
     cudaFuncSetAttribute(f16::enc0_wide_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, enc0_max);
+    io_f16::set_smem_attributes(enc0_max);               // and the 16-bit I/O forms of every unit (wunet_tc_io.cuh)
+    io_bf16::set_smem_attributes(enc0_max);
 }
 
-cudaError_t launch_enc0(cudaLaunchConfig_t cfg, int mode, const float *x, const float *w, const float *scale, const float *shift, void *out,
-                        int B, int T, int C)
+cudaError_t launch_enc0(cudaLaunchConfig_t cfg, int mode, const void *x_io, const float *w, const float *scale, const float *shift, void *out,
+                        int B, int T, int C, int io)
 {
     const int split = mode == 1 ? 1 : 0;
     const int tile = 1024 / enc0_slices(split);
     cfg.gridDim = dim3((unsigned)((T + tile - 1) / tile), (unsigned)B, 1);
     cfg.blockDim = dim3(256);
     cfg.dynamicSmemBytes = enc0_smem(C, split);
+    if (io == IO_F16) return io_f16::launch_enc0_wide(cfg, mode, x_io, w, scale, shift, out, B, T, C);
+    if (io == IO_BF16) return io_bf16::launch_enc0_wide(cfg, mode, x_io, w, scale, shift, out, B, T, C);
+    const float *x = static_cast<const float *>(x_io);
     if (mode == 2)
         return cudaLaunchKernelEx(&cfg, f16::enc0_wide_kernel<2>, x, w, scale, shift, static_cast<__half *>(out), B, T, C, 0);
     if (split)

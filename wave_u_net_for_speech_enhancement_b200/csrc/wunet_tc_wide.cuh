@@ -1,6 +1,7 @@
 // wunet_tc_wide.cuh — device code that only the wide channel plans (40 <= channels_interval <= 64) of the tensor-core inference
-// path use. Included by wunet_tc_wide.cu alone, once per element type, after wunet_tc_kernels.cuh (WUNET_TC_CONV_ONLY) in the
-// same namespace: TcElem, TcT and lrelu come from there.
+// path use. Included by wunet_tc_wide.cu (and by wunet_tc_io.cuh for the 16-bit I/O forms of enc0_wide_kernel), once per element
+// type, after wunet_tc_kernels.cuh (WUNET_TC_CONV_ONLY / WUNET_TC_IO_ONLY) in the same namespace: TcElem, TcT, TcIO and lrelu come
+// from there.
 
 // -------------------------------------------------------------------------------------------------
 // enc0 with a tile that shrinks with C
@@ -11,7 +12,7 @@
 // the folded BatchNorm, LeakyReLU and the conversions are those of enc0_kernel, so the output is the one it would write with
 // enough shared memory. No dense copy of the even rows: the row-pair form of block 1 is off for wide plans.
 template <int S>
-__global__ void __launch_bounds__(256, 3) enc0_wide_kernel(const float *__restrict__ x, const float *__restrict__ w /*[C][1][15]*/,
+__global__ void __launch_bounds__(256, 3) enc0_wide_kernel(const TcIO *__restrict__ x, const float *__restrict__ w /*[C][1][15]*/,
                                                            const float *__restrict__ scale, const float *__restrict__ shift,
                                                            TcT *__restrict__ out, int B, int T, int C, int split)
 {
@@ -31,7 +32,7 @@ __global__ void __launch_bounds__(256, 3) enc0_wide_kernel(const float *__restri
     asm volatile("griddepcontrol.wait;" ::: "memory");
     for (int i = threadIdx.x; i < TILE + 16; i += 256) {
         const int l = l0 - PAD + i - 1;
-        xs[i] = (l >= 0 && l < T) ? x[(size_t)b * T + l] : 0.f;
+        xs[i] = (l >= 0 && l < T) ? io_f32(x[(size_t)b * T + l]) : 0.f;
     }
     __syncthreads();
     float xw[20];
@@ -84,7 +85,7 @@ __global__ void __launch_bounds__(256, 3) enc0_wide_kernel(const float *__restri
     }
 }
 
-#ifndef WUNET_TC_FP16
+#if !defined(WUNET_TC_FP16) && !defined(WUNET_TC_IO_ONLY)
 // -------------------------------------------------------------------------------------------------
 // split-precision weights of the SP = 2 conv form (chunk_info): per 64-channel chunk q, positions 3q .. 3q + 2
 // -------------------------------------------------------------------------------------------------

@@ -25,11 +25,11 @@ class _PinnedPool:
     def __init__(self):
         self._buf = {}
 
-    def get(self, name: str, frames: int, sample_length: int, pin: bool) -> torch.Tensor:
-        key = (name, sample_length, pin)
+    def get(self, name: str, frames: int, sample_length: int, pin: bool, dtype: torch.dtype = torch.float32) -> torch.Tensor:
+        key = (name, sample_length, pin, dtype)
         t = self._buf.get(key)
         if t is None or t.shape[0] < frames:
-            t = torch.empty(max(frames, 1), 1, sample_length, dtype=torch.float32)
+            t = torch.empty(max(frames, 1), 1, sample_length, dtype=dtype)
             if pin:
                 t = t.pin_memory()
             self._buf[key] = t
@@ -65,24 +65,34 @@ def _ptr_array(arrays):
     return (ctypes.c_void_p * len(arrays))(*[a.ctypes.data for a in arrays])
 
 
-def frame_clips(waveforms: Sequence[np.ndarray], sample_length: int = 16384, pin: bool = True, round_to: int = 1
-                ) -> Tuple[torch.Tensor, List[Tuple[int, int, int]]]:
+_IO = {torch.float32: _lib.IO_F32, torch.float16: _lib.IO_F16, torch.bfloat16: _lib.IO_BF16}
+
+
+def frame_clips(waveforms: Sequence[np.ndarray], sample_length: int = 16384, pin: bool = True, round_to: int = 1,
+                dtype: torch.dtype = torch.float32) -> Tuple[torch.Tensor, List[Tuple[int, int, int]]]:
     """Zero-pad each 1-D waveform to a multiple of ``sample_length`` (enhancement.py:57-59) and split it into chunks
     (enhancement.py:62). Returns the stacked chunks ``[N,1,sample_length]`` (float32; a view of a pooled pinned staging
     buffer if requested, valid until the next call) and, per clip, ``(first_frame, n_frames, original_length)``.
     ``N`` is the number of chunks rounded up to a multiple of ``round_to`` (silent frames, so that every batch of the stream
     has the same size). float32 clips are copied, int16 PCM clips (a wav file's samples) are converted like the reference's
-    loader does (sample / 32768); both by the library's multi-threaded ``wunet_frame_clips_*`` (row N4)."""
+    loader does (sample / 32768); both by the library's multi-threaded ``wunet_frame_clips_*`` (row N4). ``dtype`` float16
+    or bfloat16 (a half model's input): each sample is computed in fp32 as above and rounded once to it."""
     clips, index, total = _clip_table(waveforms, sample_length)
     kinds = {c.dtype for c in clips}
     if len(kinds) > 1:
         raise ValueError("mixing int16 and float32 clips in one call is not supported")
     padded = -(-max(total, 1) // round_to) * round_to
-    frames = _POOL.get("in", padded, sample_length, pin and torch.cuda.is_available())
+    if dtype not in _IO:
+        raise ValueError(f"frames of dtype {dtype} are not supported (float32, float16, bfloat16)")
+    frames = _POOL.get("in", padded, sample_length, pin and torch.cuda.is_available(), dtype)
     lib = _lib.load()
     lens = (ctypes.c_longlong * len(clips))(*[c.shape[0] for c in clips])
-    fn = lib.wunet_frame_clips_i16 if kinds == {np.dtype(np.int16)} else lib.wunet_frame_clips_f32
-    _lib.check(fn(_ptr_array(clips), lens, len(clips), sample_length, frames.data_ptr(), padded, HOST_THREADS))
+    i16 = kinds == {np.dtype(np.int16)}
+    args = (_ptr_array(clips), lens, len(clips), sample_length, frames.data_ptr(), padded, HOST_THREADS)
+    if dtype == torch.float32:
+        _lib.check((lib.wunet_frame_clips_i16 if i16 else lib.wunet_frame_clips_f32)(*args))
+    else:
+        _lib.check((lib.wunet_frame_clips_i16_io if i16 else lib.wunet_frame_clips_f32_io)(*args, _IO[dtype]))
     return frames, index
 
 
@@ -108,18 +118,25 @@ def enhance_waveforms(model, waveforms: Sequence[np.ndarray], sample_length: int
     caller that consumes every clip at once the way enhancement.py:73-74 writes it to disk.
 
     ``model`` is a ``wave_u_net_for_speech_enhancement_b200.Model`` on a CUDA device in eval mode. ``stream_fn`` (tests
-    only) replaces ``model.forward_host_stream``."""
+    only) replaces ``model.forward_host_stream``. A half model (``model.half()`` / ``.to(torch.bfloat16)``) gets frames of
+    its dtype (half the copy bytes); its 16-bit output is widened to the float32 waveforms returned."""
     _clips, _index, total = _clip_table(waveforms, sample_length)
     B = max(1, min(batch_frames, total))
+    dtype = model._param_dtype() if hasattr(model, "_param_dtype") else None      # stream_fn tests may pass no model
+    dtype = dtype if dtype in (torch.float16, torch.bfloat16) else torch.float32
     # the batch size stays constant (one plan / workspace): the last batch is filled up with silent frames by the framing pass
-    frames, index = frame_clips(waveforms, sample_length, round_to=B)
+    frames, index = frame_clips(waveforms, sample_length, round_to=B, dtype=dtype)
     padded = frames.shape[0]
-    out = _POOL.get("out", padded, sample_length, frames.is_pinned())
+    out = _POOL.get("out", padded, sample_length, frames.is_pinned(), dtype)
     batches = [frames[i:i + B] for i in range(0, padded, B)]
     outs = [out[i:i + B] for i in range(0, padded, B)]
     fn = stream_fn if stream_fn is not None else model.forward_host_stream
     for _ in fn(batches, outs):
         pass
+    if dtype != torch.float32:
+        wide = _POOL.get("out_f32", padded, sample_length, False)
+        wide.copy_(out)                                    # exact
+        out = wide
     return unframe_clips(out, index, copy)
 
 

@@ -12,7 +12,8 @@ Surface kept identical to the reference (SURVEY §8b):
 * ``state_dict()``: the same 177 keys/shapes/dtypes, ``parameters()`` in the same registration
   order (conv.weight, conv.bias, bn.weight, bn.bias per block; encoder → middle → decoder → out), so
   reference checkpoints (``trainer/base_trainer.py:83-124``) and index-keyed Adam state interchange;
-* ``forward(input[B,1,T]) -> [B,1,T]`` fp32, T a multiple of 2**n_layers   (model/unet_basic.py:77-100)
+* ``forward(input[B,1,T]) -> [B,1,T]`` fp32, T a multiple of 2**n_layers   (model/unet_basic.py:77-100); after
+  ``model.half()`` / ``model.to(torch.bfloat16)`` the eval forward takes and returns that dtype, as the reference's modules do
 
 The sub-modules below exist ONLY as parameter/buffer containers with the reference's names; their
 ``forward`` is never called on the product path.  ``Model.forward`` hands device pointers to the
@@ -33,6 +34,11 @@ import torch.nn as nn
 from . import _lib
 
 __all__ = ["Model", "DownSamplingLayer", "UpSamplingLayer"]
+
+# element type of the eval forward's input and output -> WUNET_IO_* (a model whose parameters and buffers are all 16-bit runs
+# with 16-bit input and output, widened / rounded at the two ends of the network)
+_IO_DTYPES = {torch.float32: _lib.IO_F32, torch.float16: _lib.IO_F16, torch.bfloat16: _lib.IO_BF16}
+_HALF = (torch.float16, torch.bfloat16)
 
 
 def _conv_bn_act(cin: int, cout: int, k: int, inplace: bool) -> nn.Sequential:
@@ -353,6 +359,15 @@ class Model(nn.Module):
     ``.train()`` runs the training kernels (detached unless ``eval_autograd`` records a graph); ``forward_host`` and
     ``forward_host_stream`` refuse it. Not supported: BatchNorm with ``affine=False`` or ``track_running_stats=False``, or an
     ``eps`` other than the library's 1e-5.
+
+    Half models (no constructor argument): after ``model.half()`` or ``model.to(torch.bfloat16)`` (every parameter and buffer
+    of that one dtype) the eval forward, ``forward_host`` and ``forward_host_stream`` take an input of that dtype and return
+    one, as the reference's modules do. The computation is that of the same ``precision`` on the float32 model with the
+    parameters and samples widened to fp32 (exact), and the output rounded once to the 16-bit dtype (nearest even): so
+    ``half_model(x16) == float_model(x16.float()).to(x16.dtype)`` bit for bit. A float32 input to a half model, a 16-bit
+    input to a float32 model and mixed parameter dtypes raise RuntimeError. Training a half model (``.train()``, or an eval
+    forward that records a graph) raises too: the native training step keeps float32 parameters, and ``train_precision``
+    is how to train in 16 bits. ``read_level`` stays fp32.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
@@ -420,19 +435,29 @@ class Model(nn.Module):
         ts += [self.out[0].weight, self.out[0].bias]
         return ts
 
+    def _param_dtype(self) -> Optional[torch.dtype]:
+        """The dtype shared by every parameter and buffer the forward reads, or None when they differ."""
+        dts = {t.dtype for t in self._param_tensors()}
+        return dts.pop() if len(dts) == 1 else None
+
     def _sync_weights(self, ctx, device: torch.device):
         """(Re)pack the library's weight copies when any parameter/buffer changed: optimizer.step()
-        and load_state_dict bump ``_version``; .cpu()/.to() change ``data_ptr``."""
+        and load_state_dict bump ``_version``; .cpu()/.to()/.half() change ``data_ptr``. 16-bit parameters (all of one
+        dtype) are handed to the library as fp32 copies: widening is exact, and the library copies what it reads."""
         ds = self._state(device)
         ts = self._param_tensors()
         key = tuple((t.data_ptr(), t._version) for t in ts)
         if key == ds.weights_key:
             return
+        dtype = self._param_dtype()
         for t in ts:
             if t.device != device:
                 raise RuntimeError(f"parameter on {t.device} but input on {device}: call model.to(device) first")
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                raise RuntimeError("libwunet_b200 needs contiguous float32 parameters")
+            if dtype not in _IO_DTYPES or not t.is_contiguous():
+                raise RuntimeError("libwunet_b200 needs contiguous float32 parameters, or all of them float16 or all bfloat16 "
+                                   f"(got {', '.join(sorted({str(u.dtype) for u in ts}))})")
+        if dtype != torch.float32:
+            ts = [t.float() for t in ts]        # freed after the call: the packing kernels run on this stream first
         nb = len(self._blocks())
         arrs = []
         for slot in range(6):
@@ -515,6 +540,10 @@ class Model(nn.Module):
         buffers with its own momentum (None: the cumulative factor 1 / num_batches_tracked) and counter; in .eval() it
         normalises by the running statistics and leaves them untouched. fp32 or, with ``train_precision="bf16"`` /
         ``"tf32"`` / ``"fp16_scaled"``, bf16 / tf32 / fp16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
+        if any(t.dtype in _HALF for t in self._param_tensors()):
+            raise RuntimeError("libwunet_b200 needs contiguous float32 parameters on the input's device: the native training "
+                               "step keeps float32 parameters. To train in 16 bits, train the float32 model with "
+                               "Model(train_precision='bf16' or 'fp16_scaled') and call .half() / .to(torch.bfloat16) to deploy it.")
         self._check_input(x)
         B, _, T = x.shape
         blocks = self._blocks()
@@ -582,10 +611,14 @@ class Model(nn.Module):
         return lambda buf: dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
 
     def _check_input(self, x: torch.Tensor):
+        """[B, 1, T], and float32 unless the parameters are all float16 (or all bfloat16): then of that dtype."""
         if x.dim() != 3 or x.size(1) != 1:
             raise RuntimeError(f"expected input of shape [B, 1, T], got {tuple(x.shape)}")
-        if x.dtype != torch.float32:
-            raise RuntimeError(f"expected float32 input, got {x.dtype}")
+        pd = self._param_dtype()
+        want = pd if pd in _HALF else torch.float32
+        if x.dtype != want:
+            raise RuntimeError(f"expected {str(want).replace('torch.', '')} input for a model whose parameters are "
+                               f"{'of mixed dtypes' if pd is None else pd}, got {x.dtype}")
 
     @staticmethod
     def _aligned(x: torch.Tensor) -> torch.Tensor:
@@ -623,14 +656,16 @@ class Model(nn.Module):
             ws = self._workspace(ctx, B, T, prec, x.device)
             y = torch.empty_like(x)
             stream = torch.cuda.current_stream(x.device).cuda_stream
-            _lib.check(lib.wunet_forward(ctx, x.data_ptr(), y.data_ptr(), B, T, prec, ws.data_ptr(), ws.numel(), stream))
+            _lib.check(lib.wunet_forward_io(ctx, x.data_ptr(), y.data_ptr(), B, T, prec, _IO_DTYPES[x.dtype], ws.data_ptr(),
+                                            ws.numel(), stream))
         return y
 
     @torch.no_grad()
     def forward_host(self, x_host: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """End-to-end form of enhancement.py:64-66 (``model(chunk).detach().cpu()``): host tensor in,
-        host tensor out; H2D copy, kernels and D2H copy are enqueued by ``wunet_forward_host``.
-        Parameters must already live on a CUDA device. Pinned tensors give full copy bandwidth."""
+        host tensor out; H2D copy, kernels and D2H copy are enqueued by ``wunet_forward_host_io``.
+        Parameters must already live on a CUDA device. Pinned tensors give full copy bandwidth. A 16-bit model takes and
+        returns 16-bit tensors (half the copy bytes)."""
         self._check_input(x_host)
         if x_host.is_cuda:
             raise RuntimeError("forward_host takes a host tensor")
@@ -651,16 +686,17 @@ class Model(nn.Module):
             cur = torch.cuda.current_stream(device)
             self._sync_weights(ctx, device)
             cur.synchronize()                      # packing ran on torch's stream; forward_host uses its own
-            _lib.check(_lib.load().wunet_forward_host(ctx, x_host.data_ptr(), out.data_ptr(), B, T,
-                                                      _lib.PRECISIONS[self.precision]))
+            _lib.check(_lib.load().wunet_forward_host_io(ctx, x_host.data_ptr(), out.data_ptr(), B, T,
+                                                         _lib.PRECISIONS[self.precision], _IO_DTYPES[x_host.dtype]))
         return out
 
     @torch.no_grad()
     def forward_host_stream(self, batches, outs=None):
         """Streaming form of :meth:`forward_host` for many host batches (every chunk of every clip, enhancement.py:49-74):
         yields one output tensor per input batch, in order; H2D copy, kernels and D2H copy of consecutive batches overlap
-        (two batches in flight). ``batches``: iterable of pinned ``[B,1,T]`` float32 host tensors that must stay alive until
-        their result has been yielded; ``outs``: optional iterable of pinned output tensors."""
+        (two batches in flight). ``batches``: iterable of pinned ``[B,1,T]`` host tensors (float32, or the dtype of a 16-bit
+        model) that must stay alive until their result has been yielded; ``outs``: optional iterable of pinned output
+        tensors of the same dtype."""
         if self.training or self._bn_any_training():
             raise NotImplementedError("forward_host_stream is eval-only (model and every BatchNorm container in .eval())")
         device = self.out[0].weight.device
@@ -682,7 +718,10 @@ class Model(nn.Module):
                 out = next(outs_it) if outs_it is not None else torch.empty_like(x, pin_memory=x.is_pinned())
                 B, _, T = x.shape
                 ticket = ctypes.c_int(0)
-                _lib.check(lib.wunet_stream_submit(ctx, x.data_ptr(), out.data_ptr(), B, T, prec, ctypes.byref(ticket)))
+                if out.dtype != x.dtype:
+                    raise RuntimeError(f"output buffer is {out.dtype}, the input {x.dtype}")
+                _lib.check(lib.wunet_stream_submit_io(ctx, x.data_ptr(), out.data_ptr(), B, T, prec, _IO_DTYPES[x.dtype],
+                                                      ctypes.byref(ticket)))
                 pending.append((ticket.value, x, out))
                 if len(pending) == 2:
                     t, _x, o = pending.pop(0)
