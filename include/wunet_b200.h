@@ -120,6 +120,23 @@ int wunet_forward_io(wunet_ctx *ctx, const void *x_dev, void *y_dev, int B, int 
                      void *workspace, size_t workspace_bytes, void *stream);
 
 /*
+ * wunet_forward_io that also writes the outputs of chosen blocks: what forward hooks on the reference's encoder[i], middle and
+ * decoder[j] see (model/unet_basic.py:82-96), for the Python module's hooks on those containers.
+ *   export_mask[2n+1] (forward order: encoder 0 .. n-1, middle, decoder 0 .. n-1; NULL or all zero = wunet_forward_io, the same
+ *     launches and bits): a nonzero entry i writes block i's full-resolution output to level_out[i] (device, caller-owned) as
+ *     [B][Cout][L] of io_dtype. The value is the block output the next block reads, widened exactly to fp32 (fp32_tc: hi + lo of
+ *     its split halves) and, for 16-bit I/O, rounded once to io_dtype (nearest even); with WUNET_IO_F32 it equals
+ *     wunet_read_level's bit for bit.
+ *   The last decoder block is fused with the head and stores no output on the tensor-core precisions; when it is marked, the
+ *     same kernel runs with its activation store switched on (its launch and y are unchanged, bit for bit).
+ *   One conversion launch per marked block after the forward, on `stream`; wunet_last_launch_count() counts the forward only.
+ *   The workspace is wunet_workspace_bytes()'s. A marked block without a buffer -> WUNET_EINVAL before anything is enqueued.
+ */
+int wunet_forward_export(wunet_ctx *ctx, const void *x_dev, void *y_dev, int B, int T, int precision, int io_dtype,
+                         const unsigned char *export_mask, void *const *level_out, void *workspace, size_t workspace_bytes,
+                         void *stream);
+
+/*
  * Same operator with HOST buffers (the end-to-end form used by enhancement.py:64-66, which does
  * `model(chunk).detach().cpu()`): copies x_host -> device, runs the forward, copies y back and
  * waits for it.  Uses context-owned, grow-only device buffers and a context-owned stream.
@@ -333,6 +350,22 @@ int wunet_train_backward_blocks(wunet_ctx *ctx, const float *x, const float *y, 
                                 const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
                                 float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                                 void *stream, float *dx, int part, int precision, int flags, const unsigned char *bn_frozen);
+/* wunet_train_backward_blocks with extra upstream gradients of block outputs: the gradients that flow back into what forward
+ * hooks on the reference's encoder[i], middle and decoder[j] captured (feature-matching, deep-supervision or distillation
+ * losses on intermediate levels).
+ *   g_act[2n+1] (forward order; NULL, or a NULL entry = none): device [B][Cout][L] fp32, the gradient of the loss with respect to
+ *     block i's output (its activation after LeakyReLU). It is added, element by element, to the gradient that reaches that
+ *     output from the rest of the network (the next block, the decoder's skip, the head), right before block i's BatchNorm
+ *     backward, so deterministic mode stays bitwise repeatable and under WUNET_PREC_FP16_SCALED the block's max |dz| includes it.
+ *   It is added in the part that processes block i (encoders and middle: part 1, decoders: part 0), and only at or above the
+ *     early stop: parameter-gradient and dx requests decide where the backward stops, as in wunet_train_backward_blocks.
+ *   With every entry NULL this is wunet_train_backward_blocks: the same launches. */
+int wunet_train_backward_inject(wunet_ctx *ctx, const float *x, const float *y, const float *dy, int B, int T,
+                                const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                                const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                                float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                                void *stream, float *dx, int part, int precision, int flags, const unsigned char *bn_frozen,
+                                const float *const *g_act);
 /* BatchNorm statistics synchronised over data-parallel ranks: what nn.SyncBatchNorm (torch.nn.SyncBatchNorm.
  * convert_sync_batchnorm(model)) computes in a one-process-per-GPU step. With a hook installed, every training forward with
  * batch statistics (not WUNET_TRAIN_FROZEN_BN) on this context, and its backward, compute the BatchNorm reductions from sums

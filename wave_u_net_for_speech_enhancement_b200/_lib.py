@@ -64,6 +64,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_forward_host_io.argtypes = [vp, vp, vp, ci, ci, ci, ci]
     lib.wunet_stream_submit_io.argtypes = [vp, vp, vp, ci, ci, ci, ci, ctypes.POINTER(ci)]
     lib.wunet_read_level.argtypes = [vp, ci, vp, ci, ci, ci, vp, vp]
+    lib.wunet_forward_export.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, vp, vp, cs, vp]
     ll = ctypes.c_longlong
     lib.wunet_frame_clips_f32.argtypes = [vp, vp, ci, ci, vp, ll, ci]
     lib.wunet_frame_clips_i16.argtypes = [vp, vp, ci, ci, vp, ll, ci]
@@ -94,6 +95,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_train_backward_ex.argtypes = lib.wunet_train_backward.argtypes + [vp, ci, ci, ci]
     lib.wunet_train_forward_blocks.argtypes = lib.wunet_train_forward_ex.argtypes + [vp, vp]
     lib.wunet_train_backward_blocks.argtypes = lib.wunet_train_backward_ex.argtypes + [vp]
+    lib.wunet_train_backward_inject.argtypes = lib.wunet_train_backward_blocks.argtypes + [vp]
     lib.wunet_train_set_bn_allreduce.argtypes = [vp, BN_ALLREDUCE_FN, vp, vp, cs]
     lib.wunet_debug_train_conv.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     lib.wunet_debug_train_layout.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ll), ci]
@@ -119,6 +121,7 @@ EXPORTED_SYMBOLS = [
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
     "wunet_forward_io", "wunet_forward_host_io", "wunet_stream_submit_io", "wunet_frame_clips_f32_io", "wunet_frame_clips_i16_io",
+    "wunet_forward_export", "wunet_train_backward_inject",
 ]
 
 PLAN_FIELDS = ["L", "Cin0", "Cin1", "Cout", "Npad", "Nh", "nsplit", "Nstride", "MT", "nacc", "packed", "FR", "S", "m_tiles",

@@ -321,8 +321,9 @@ int wunet_forward(wunet_ctx *c, const float *x, float *y, int B, int T, int prec
     return wunet_forward_io(c, x, y, B, T, precision, WUNET_IO_F32, workspace, workspace_bytes, stream);
 }
 
-int wunet_forward_io(wunet_ctx *c, const void *x, void *y, int B, int T, int precision, int io, void *workspace,
-                     size_t workspace_bytes, void *stream)
+// wunet_forward_io; store_last: the tensor-core forward also stores the last decoder block (wunet_forward_export)
+static int forward_io_impl(wunet_ctx *c, const void *x, void *y, int B, int T, int precision, int io, void *workspace,
+                           size_t workspace_bytes, void *stream, bool store_last)
 {
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
@@ -338,10 +339,50 @@ int wunet_forward_io(wunet_ctx *c, const void *x, void *y, int B, int T, int pre
     int launches = 0;
     cudaEvent_t *ev = prof_events(c);
     if (tc_mode(precision) < 0) return fail(WUNET_EINVAL, "unknown precision %d", precision);
-    const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, tc_mode(precision), io);
+    const int r = tc_forward(c->tc, x, y, B, T, workspace, st, &launches, ev, tc_mode(precision), io, store_last);
     if (ev && r == 0) c->ev_recorded = 2 * c->n + 3;
     if (r != 0) return fail(WUNET_ECUDA, "tensor-core forward failed: %s", tc_error());
     c->last_launches = launches;
+    return WUNET_OK;
+}
+
+int wunet_forward_io(wunet_ctx *c, const void *x, void *y, int B, int T, int precision, int io, void *workspace,
+                     size_t workspace_bytes, void *stream)
+{
+    return forward_io_impl(c, x, y, B, T, precision, io, workspace, workspace_bytes, stream, false);
+}
+
+int wunet_forward_export(wunet_ctx *c, const void *x, void *y, int B, int T, int precision, int io,
+                         const unsigned char *export_mask, void *const *level_out, void *workspace, size_t workspace_bytes,
+                         void *stream)
+{
+    if (!c) return fail(WUNET_EINVAL, "null context");
+    const int nb = 2 * c->n + 1;
+    bool any = false;
+    for (int i = 0; export_mask && i < nb; ++i) {
+        if (!export_mask[i]) continue;
+        if (!level_out || !level_out[i]) return fail(WUNET_EINVAL, "block %d is marked for export but has no output buffer", i);
+        any = true;
+    }
+    const bool last = any && export_mask[nb - 1];
+    int rc = forward_io_impl(c, x, y, B, T, precision, io, workspace, workspace_bytes, stream, last);
+    if (rc != WUNET_OK || !any) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    std::vector<size_t> off;
+    size_t total;
+    if (precision == WUNET_PREC_FP32) fp32_layout(c, B, T, off, total);
+    for (int i = 0; i < nb; ++i) {
+        if (!export_mask[i]) continue;
+        const int C = c->blocks[i].cout, L = level_len(c, i, T);
+        if (precision != WUNET_PREC_FP32) {
+            if (tc_export_level(c->tc, i, workspace, B, T, level_out[i], io, st, tc_mode(precision)) != 0)
+                return fail(WUNET_ECUDA, "block %d export failed: %s", i, tc_error());
+        } else if (io == WUNET_IO_F32) {
+            CUDA_TRY(cudaMemcpyAsync(level_out[i], static_cast<const char *>(workspace) + off[i], (size_t)B * C * L * sizeof(float),
+                                     cudaMemcpyDeviceToDevice, st));
+        } else if (launch_level_export_io(static_cast<const char *>(workspace) + off[i], LEVEL_F32_NCL, level_out[i], io, B, L, C, st) < 0)
+            return fail(WUNET_ECUDA, "block %d export launch failed: %s", i, cudaGetErrorString(cudaGetLastError()));
+    }
     return WUNET_OK;
 }
 
@@ -657,7 +698,7 @@ static int train_backward_impl(wunet_ctx *c, const float *x, const float *y, con
                                const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
                                float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
                                void *stream, float *dx, int part, int precision, int flags, bool blocks,
-                               const unsigned char *bn_frozen)
+                               const unsigned char *bn_frozen, const float *const *g_act = nullptr)
 {
     int rc = check_shape(c, B, T);
     if (rc != WUNET_OK) return rc;
@@ -682,7 +723,7 @@ static int train_backward_impl(wunet_ctx *c, const float *x, const float *y, con
     }
     const bool synced = c->bn_sync.fn && any_batch;
     if (train_backward(c->n, c->ci, x, y, dy, B, T, P, G, workspace, static_cast<cudaStream_t>(stream), part, prec, dx, tflags,
-                       synced ? &c->bn_sync : nullptr, bn_frozen, blocks))
+                       synced ? &c->bn_sync : nullptr, bn_frozen, blocks, g_act))
         return fail(WUNET_ECUDA, "%s", train_error());
     return WUNET_OK;
 }
@@ -705,6 +746,18 @@ int wunet_train_backward_blocks(wunet_ctx *c, const float *x, const float *y, co
 {
     return train_backward_impl(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight, g_bn_bias,
                                g_out_w, g_out_b, workspace, workspace_bytes, stream, dx, part, precision, flags, true, bn_frozen);
+}
+
+int wunet_train_backward_inject(wunet_ctx *c, const float *x, const float *y, const float *dy, int B, int T,
+                                const float *const *conv_w, const float *const *bn_weight, const float *const *bn_bias,
+                                const float *out_w, float *const *g_conv_w, float *const *g_conv_b, float *const *g_bn_weight,
+                                float *const *g_bn_bias, float *g_out_w, float *g_out_b, void *workspace, size_t workspace_bytes,
+                                void *stream, float *dx, int part, int precision, int flags, const unsigned char *bn_frozen,
+                                const float *const *g_act)
+{
+    return train_backward_impl(c, x, y, dy, B, T, conv_w, bn_weight, bn_bias, out_w, g_conv_w, g_conv_b, g_bn_weight, g_bn_bias,
+                               g_out_w, g_out_b, workspace, workspace_bytes, stream, dx, part, precision, flags, true, bn_frozen,
+                               g_act);
 }
 
 int wunet_train_set_bn_allreduce(wunet_ctx *c, wunet_bn_allreduce_fn fn, void *user, double *buf, size_t capacity)

@@ -145,4 +145,13 @@ int train_tc_pack_f16(const float *w, void *wf, void *wb, int Cout, int Cin, int
 int launch_train_conv_tc_f16(const ConvArgs &a, int ksize, int mode, cudaStream_t st);
 int launch_train_wgrad_tc_f16(const ConvArgs &a, const float *dz, float *dw, int ksize, int mode, cudaStream_t st, bool slices);
 
+// ---- block forward hooks, implemented in wunet_hooks.cu ---------------------------------------------------------------------
+// How a block output is stored in an inference workspace: channels-last bf16 or fp16 [B][L][C], the split-precision [B][L][hi C |
+// lo C] bf16 halves, or fp32 [B][C][L] (the fp32 path).
+enum LevelKind : int { LEVEL_BF16 = 0, LEVEL_SPLIT = 1, LEVEL_F16 = 2, LEVEL_F32_NCL = 3 };
+// dst [B][C][L] of IoType io (IO_F16 or IO_BF16): each element widened exactly to fp32, then rounded once to io. 1 launch, or -1.
+int launch_level_export_io(const void *src, int kind, void *dst, int io, int B, int L, int C, cudaStream_t st);
+// ga[0 .. n) += g[0 .. n), element by element. 1 launch, or -1.
+int launch_grad_inject(float *ga, const float *g, long long n, cudaStream_t st);
+
 }  // namespace wunet

@@ -1001,7 +1001,7 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
 }
 
 static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const void *x = nullptr, void *y = nullptr,
-                        int io = IO_F32);
+                        int io = IO_F32, void *out = nullptr);
 
 // enc0 over frames [f0, f0 + nf) of x (IoType io samples: the 16-bit forms are those of wunet_tc_io.cuh); *launches receives the
 // number of kernels enqueued
@@ -1061,8 +1061,9 @@ static int launch_enc0(TcState *st, const void *x_io, int f0, int nf, int T, voi
     return 0;
 }
 
-// conv block i over the tile range [t0, t1) (t1 < 0: all tiles)
-static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const void *x, void *y, int io)
+// conv block i over the tile range [t0, t1) (t1 < 0: all tiles); out: null, or where the last block (fused with the head, which
+// stores no activation by default) also stores its output, in the layout of the other blocks
+static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream, const void *x, void *y, int io, void *out)
 {
     TcPlanLevel &P = st->plan.lv[i];
     if (P.is_gemm) {
@@ -1080,6 +1081,7 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
     TcParams p = P.p;
     p.x = static_cast<const float *>(x); p.y = static_cast<float *>(y);   // only the fused head (last block) reads x / writes y (IO samples)
     p.pf_late = st->pf_late ? 1 : 0;
+    if (out) p.out = out;
     if (t1 >= 0) { p.tile_begin = t0; p.tile_end = t1; }
     const int ntiles = p.tile_end - p.tile_begin;
     cudaLaunchConfig_t cfg{};
@@ -1125,7 +1127,7 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
 }
 
 int tc_forward(TcState *st, const void *x, void *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
-               cudaEvent_t *ev, int mode, int io)
+               cudaEvent_t *ev, int mode, int io, bool store_last)
 {
     if (tc_prepare(st, nullptr, nullptr, B, T, ws, mode, stream)) return -1;
     const int n = st->n;
@@ -1136,7 +1138,8 @@ int tc_forward(TcState *st, const void *x, void *y, int B, int T, void *ws, cuda
     nl += l0n;
     if (ev) cudaEventRecord(ev[1], stream);
     for (int i = 1; i < 2 * n + 1; ++i) {
-        if (launch_block(st, i, 0, -1, stream, x, y, io)) return -1;
+        void *out = (store_last && i == 2 * n) ? static_cast<char *>(ws) + st->plan.off[i] : nullptr;
+        if (launch_block(st, i, 0, -1, stream, x, y, io, out)) return -1;
         ++nl;
         if (ev) cudaEventRecord(ev[i + 1], stream);
     }
@@ -1201,9 +1204,15 @@ int tc_forward_host(TcState *st, const void *x_host, void *y_host, void *x_dev, 
 int tc_read_level(TcState *st, int block, const void *ws, int B, int T, float *out_ncl, cudaStream_t stream, int mode)
 {
     if (!st) return tc_fail("tensor-core state missing");
-    const int n = st->n;
-    if (block == 2 * n && !st->store_last)
+    if (block == 2 * st->n && !st->store_last)
         return tc_fail("the last decoder block is fused with the head and not materialised (set WUNET_TC_STORE_LAST=1)");
+    return tc_export_level(st, block, ws, B, T, out_ncl, IO_F32, stream, mode);
+}
+
+int tc_export_level(TcState *st, int block, const void *ws, int B, int T, void *out_ncl, int io, cudaStream_t stream, int mode)
+{
+    if (!st) return tc_fail("tensor-core state missing");
+    const int n = st->n;
     std::vector<size_t> off;
     size_t total;
     tc_layout(n, st->ci, B, T, off, total, mode);
@@ -1211,9 +1220,12 @@ int tc_read_level(TcState *st, int block, const void *ws, int B, int T, float *o
     const int C = st->levels[block].cout;
     const long long nel = (long long)B * C * L;
     const __nv_bfloat16 *src = reinterpret_cast<const __nv_bfloat16 *>(static_cast<const char *>(ws) + off[block]);
-    if (mode == 2) return f16::nlc_to_ncl(src, out_ncl, B, L, C, stream) == cudaSuccess ? 0 : tc_fail("read_level launch failed");
-    if (mode == 1) nlc_split_to_ncl_f32_kernel<<<(unsigned)((nel + 255) / 256), 256, 0, stream>>>(src, out_ncl, B, L, C);
-    else nlc_bf16_to_ncl_f32_kernel<<<(unsigned)((nel + 255) / 256), 256, 0, stream>>>(src, out_ncl, B, L, C);
+    if (io != IO_F32)      // LevelKind == mode
+        return launch_level_export_io(src, mode, out_ncl, io, B, L, C, stream) > 0 ? 0 : tc_fail("level export launch failed");
+    float *dst = static_cast<float *>(out_ncl);
+    if (mode == 2) return f16::nlc_to_ncl(src, dst, B, L, C, stream) == cudaSuccess ? 0 : tc_fail("read_level launch failed");
+    if (mode == 1) nlc_split_to_ncl_f32_kernel<<<(unsigned)((nel + 255) / 256), 256, 0, stream>>>(src, dst, B, L, C);
+    else nlc_bf16_to_ncl_f32_kernel<<<(unsigned)((nel + 255) / 256), 256, 0, stream>>>(src, dst, B, L, C);
     return cudaGetLastError() == cudaSuccess ? 0 : tc_fail("read_level launch failed");
 }
 

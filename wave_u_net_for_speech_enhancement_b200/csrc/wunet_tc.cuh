@@ -24,12 +24,16 @@ int tc_set_weights(TcState **st, int n_layers, int ci, const TcBlockSrc *blocks,
 size_t tc_workspace_bytes(int n_layers, int ci, int B, int T, int mode = 0);
 // events: null, or 2n+3 events: [0] before the first kernel, [i+1] after block i, [2n+2] after the head
 // x, y: B*T samples of the IoType io (wunet_common.cuh)
+// store_last: the last decoder block, fused with the head, also stores its output to its workspace slot (y is unchanged)
 int tc_forward(TcState *st, const void *x, void *y, int B, int T, void *ws, cudaStream_t stream, int *launches,
-               cudaEvent_t *events, int mode = 0, int io = 0);
+               cudaEvent_t *events, int mode = 0, int io = 0, bool store_last = false);
 // host-buffer form: x_host/y_host (pinned for full rate), x_dev/y_dev = device staging buffers of B*T samples of the IoType io
 int tc_forward_host(TcState *st, const void *x_host, void *y_host, void *x_dev, void *y_dev, int B, int T, void *ws,
                     cudaStream_t stream, int *launches, int mode = 0, int io = 0);
 int tc_read_level(TcState *st, int block, const void *ws, int B, int T, float *out_ncl, cudaStream_t stream, int mode = 0);
+// block output `block` of the last forward on ws as [B][C][L] of the IoType io (fp32: tc_read_level's kernels; 16-bit: widened
+// exactly, rounded once). The caller knows that the block was stored (the last one only with store_last or WUNET_TC_STORE_LAST).
+int tc_export_level(TcState *st, int block, const void *ws, int B, int T, void *out_ncl, int io, cudaStream_t stream, int mode);
 void tc_destroy(TcState *st);
 // host-only: the tiling build_plan would choose for `block` (32 ints, see wunet_debug_plan in include/wunet_b200.h); mode 1 =
 // the split-precision (fp32_tc) plan; mode 2 (fp16) = the bf16 plan

@@ -938,7 +938,7 @@ int train_forward(int n, int ci, const float *x, float *y, int B, int T, const T
 
 int train_backward(int n, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
                    const TrainGrads &G, void *workspace, cudaStream_t st, int part, int prec, float *dx, int flags,
-                   const BnSync *sync, const unsigned char *bn_frozen, bool early_stop)
+                   const BnSync *sync, const unsigned char *bn_frozen, bool early_stop, const float *const *g_act)
 {
     std::vector<Shape> sh;
     shapes_of(n, ci, T, sh);
@@ -997,6 +997,10 @@ int train_backward(int n, int ci, const float *x, const float *y, const float *d
         const long long nel = (long long)B * s.cout * s.L;
         float *g_gamma = slot(G.bn_w, i), *g_beta = slot(G.bn_b, i), *g_cb = slot(G.conv_b, i), *g_cw = slot(G.conv_w, i);
         const bool frozen = frozen_at(i);
+        // a forward hook's upstream gradient of this block's output: ga is complete here (head or upsample adjoint, skip and
+        // decimation adjoints), so the sum is the same whatever the launch order of the others
+        if (g_act && g_act[i] && launch_grad_inject(ga, g_act[i], nel, st) < 0)
+            return train_fail("training backward, block %d: gradient injection launch failed", i);
         // batch statistics: dz needs mean(dy) and mean(dy zh) (s1, s2); frozen statistics: they are constants, dz = invstd
         // gamma dy (s1 = s2 = 0), and the reductions only serve the BatchNorm parameter gradients
         if (sync && !frozen) {

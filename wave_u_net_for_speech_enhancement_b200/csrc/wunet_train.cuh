@@ -79,10 +79,12 @@ int train_forward(int n_layers, int ci, const float *x, float *y, int B, int T, 
 // bn_frozen: as in the forward. A null array or entry in G is a frozen parameter: nothing is computed for it or written.
 // early_stop: nothing is issued below the lowest block that needs a gradient (or dx), and that block skips its input
 // gradient; dx then also goes to part 0, unwritten, to say that part 1 will ask for it.
+// g_act: null, or 2n+1 device pointers (null = none): g_act[i] [B][Cout][L] is added to block i's activation gradient before its
+// BatchNorm backward, when block i is processed (its part, at or above the early stop).
 int train_backward(int n_layers, int ci, const float *x, const float *y, const float *dy, int B, int T, const TrainParams &P,
                    const TrainGrads &G, void *workspace, cudaStream_t stream, int part = -1, int prec = TRAIN_FP32,
                    float *dx = nullptr, int flags = 0, const BnSync *sync = nullptr, const unsigned char *bn_frozen = nullptr,
-                   bool early_stop = false);
+                   bool early_stop = false, const float *const *g_act = nullptr);
 // One convolution-shaped pass on caller device buffers (test hook): pass 0 = forward conv out[B][Cout][L] = conv(in, w);
 // 1 = input gradient out[B][Cin][L] of dz [B][Cout][L] (Conv1d padding, no mode); 2 = weight gradient out[Cout][Cin][K] =
 // sum dz * in. `in` is built from src0 / src1 per `mode` as in the forward (ConvArgs). Synchronous.

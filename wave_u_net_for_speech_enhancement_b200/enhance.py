@@ -119,7 +119,8 @@ def enhance_waveforms(model, waveforms: Sequence[np.ndarray], sample_length: int
 
     ``model`` is a ``wave_u_net_for_speech_enhancement_b200.Model`` on a CUDA device in eval mode. ``stream_fn`` (tests
     only) replaces ``model.forward_host_stream``. A half model (``model.half()`` / ``.to(torch.bfloat16)``) gets frames of
-    its dtype (half the copy bytes); its 16-bit output is widened to the float32 waveforms returned."""
+    its dtype (half the copy bytes); its 16-bit output is widened to the float32 waveforms returned. It streams through
+    ``Model.forward_host_stream``, not ``forward``: forward hooks on the model's blocks do not fire."""
     _clips, _index, total = _clip_table(waveforms, sample_length)
     B = max(1, min(batch_frames, total))
     dtype = model._param_dtype() if hasattr(model, "_param_dtype") else None      # stream_fn tests may pass no model

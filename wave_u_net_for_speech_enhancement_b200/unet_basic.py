@@ -30,6 +30,9 @@ from typing import Dict, Optional, Tuple
 import torch
 import torch.distributed as dist
 import torch.nn as nn
+import torch.nn.functional as F
+from torch.nn.modules import module as _nn_module
+from torch.utils.hooks import RemovableHandle
 
 from . import _lib
 
@@ -185,7 +188,12 @@ class _NativeTrainStep(torch.autograd.Function):
     only (no weight-gradient pass, no reduction, no all-reduce).
 
     ``reducer``: None, or the callable that sums a float64 CUDA view over the data-parallel ranks in place (nn.SyncBatchNorm):
-    the forward's batch statistics and its backward's BatchNorm means then cover every rank's frames."""
+    the forward's batch statistics and its backward's BatchNorm means then cover every rank's frames.
+
+    ``export``: the blocks (forward order, 0 .. 2n) whose outputs the forward also returns, after ``y``, as fp32 [B, Cout, L]
+    copies of the activations the workspace holds (what forward hooks on the block containers see). The gradients that reach
+    them are added to those blocks' activation gradients inside the backward (wunet_train_backward_inject). Empty: the
+    Function returns ``y`` alone and its backward makes exactly the calls it makes without hooks."""
 
     @staticmethod
     def _ptr_array(tensors):
@@ -193,6 +201,10 @@ class _NativeTrainStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, flags, reducer, blocks_state, x, *params):
+        return _NativeTrainStep._forward(ctx, model, flags, reducer, blocks_state, (), x, params)
+
+    @staticmethod
+    def _forward(ctx, model, flags, reducer, blocks_state, export, x, params):
         lib = _lib.load()
         blocks = model._blocks()
         nb = len(blocks)
@@ -228,23 +240,37 @@ class _NativeTrainStep(torch.autograd.Function):
                 bn_frozen = (ctypes.c_ubyte * nb)(*[1 if f else 0 for f in frozen])
                 _native_call(lib, c, reducer, bn_buf, lambda: lib.wunet_train_forward_blocks(
                     *args, 0.0, ws.data_ptr(), ws.numel(), stream, prec, flags, bn_frozen, (ctypes.c_float * nb)(*momenta)))
+            levels = []
+            for i in export:                                 # copies of the activations, fp32 [B, Cout, L]
+                lay = _lib.debug_train_layout(model.n_layers, model.channels_interval, B, T, i, model.train_precision)
+                nel = B * lay["Cout"] * lay["L"]
+                levels.append(ws[lay["act"]:lay["act"] + 4 * nel].view(torch.float32).view(B, lay["Cout"], lay["L"]).clone())
         # the backward runs at the precision, BatchNorm mode and synchronisation of ITS forward (and reads the bf16 weight
         # packings that forward left in ws)
         ctx.model, ctx.ws, ctx.nb, ctx.prec, ctx.flags = model, ws, nb, prec, flags
-        ctx.reducer, ctx.bn_buf, ctx.bn_frozen = reducer, bn_buf, bn_frozen
+        ctx.reducer, ctx.bn_buf, ctx.bn_frozen, ctx.export = reducer, bn_buf, bn_frozen, export
+        ctx.x_arg = 5 if export else 4                       # position of x among apply()'s arguments
         ctx.save_for_backward(x, y, *params)
-        return y
+        if not export:
+            return y
+        ctx.set_materialize_grads(False)                     # a level the loss does not use has no gradient to add
+        return (y, *levels)
 
     @staticmethod
-    def backward(ctx, gy):
+    def backward(ctx, gy, *g_levels):
         from .train_step import GradientBucket, data_parallel_world
         lib = _lib.load()
         x, y, *params = ctx.saved_tensors
         nb = ctx.nb
         B, _, T = x.shape
-        gy = gy.contiguous()
-        want_dx = ctx.needs_input_grad[4]
-        mask = ctx.needs_input_grad[5:]
+        gy = torch.zeros_like(y) if gy is None else gy.contiguous()
+        g_act = [None] * nb                                  # upstream gradients of the exported block outputs
+        for i, g in zip(ctx.export, g_levels):
+            if g is not None:
+                g_act[i] = g.float().contiguous()
+        inject = any(g is not None for g in g_act)
+        want_dx = ctx.needs_input_grad[ctx.x_arg]
+        mask = ctx.needs_input_grad[ctx.x_arg + 1:]
         want_params = any(mask)
         per_block = ctx.bn_frozen is not None              # the forward ran wunet_train_forward_blocks
         dx = torch.empty_like(x) if want_dx else None
@@ -269,7 +295,11 @@ class _NativeTrainStep(torch.autograd.Function):
                 args = (c, x.data_ptr(), y.data_ptr(), gy.data_ptr(), B, T, P(sel(params, 0)), P(sel(params, 2)), P(sel(params, 3)),
                         params[-2].data_ptr(), G(0), G(1), G(2), G(3), ptr(grads[-2]), ptr(grads[-1]), ctx.ws.data_ptr(),
                         ctx.ws.numel(), stream)
-                if per_block:
+                if inject:
+                    # each block's hook gradient is added in the part that processes the block; dx goes to part 0 as well, as below
+                    _native_call(lib, c, ctx.reducer, ctx.bn_buf, lambda: lib.wunet_train_backward_inject(
+                        *args, ptr(dx), part, ctx.prec, flags, ctx.bn_frozen, P(g_act)))
+                elif per_block:
                     # dx goes to part 0 as well: it tells the early stop that part 1 will need the gradient of block 0
                     _native_call(lib, c, ctx.reducer, ctx.bn_buf, lambda: lib.wunet_train_backward_blocks(
                         *args, ptr(dx), part, ctx.prec, flags, ctx.bn_frozen))
@@ -282,7 +312,16 @@ class _NativeTrainStep(torch.autograd.Function):
             if reduce:
                 bucket.finish()
         ctx.ws = ctx.bn_buf = ctx.reducer = ctx.bn_frozen = None
-        return (None, None, None, None, dx, *grads)          # none for the model handle, the flags, the reducer, the block state
+        # none for the model handle, the flags, the reducer, the block state (and the exported blocks)
+        return (*[None] * ctx.x_arg, dx, *grads)
+
+
+class _NativeTrainStepExport(_NativeTrainStep):
+    """:class:`_NativeTrainStep` that also returns the outputs of the blocks ``export`` (a non-empty tuple), for forward hooks."""
+
+    @staticmethod
+    def forward(ctx, model, flags, reducer, blocks_state, export, x, *params):
+        return _NativeTrainStep._forward(ctx, model, flags, reducer, blocks_state, export, x, params)
 
 
 class Model(nn.Module):
@@ -368,6 +407,23 @@ class Model(nn.Module):
     input to a float32 model and mixed parameter dtypes raise RuntimeError. Training a half model (``.train()``, or an eval
     forward that records a graph) raises too: the native training step keeps float32 parameters, and ``train_precision``
     is how to train in 16 bits. ``read_level`` stays fp32.
+
+    Forward hooks (no constructor argument): ``register_forward_hook`` (``with_kwargs`` and ``always_call`` included) on
+    ``encoder[i]``, ``encoder[i].main``, ``middle``, ``decoder[j]``, ``decoder[j].main`` and ``out``, and global module forward
+    hooks, fire from the native forward in the reference's order (encoder 0 .. n-1, middle, decoder 0 .. n-1, out; a block's
+    ``main`` before the block) after its kernels are enqueued and before ``forward`` returns. A hook receives ``(module,
+    (input,), output)`` with the reference's meaning: the block's full-resolution output [B, Cout, L] (an encoder's before
+    decimation; ``out``: the model output), and as input x, the previous output ``[:, :, ::2]`` or, for a decoder block,
+    ``cat([F.interpolate(prev, scale_factor=2, mode="linear", align_corners=True), skip])`` computed with torch from the
+    exported outputs (torch's arithmetic). Outputs are fresh tensors of the model's dtype: at the inference precisions the block
+    output the next block reads, widened to fp32 and, for a half model, rounded once; in the training kernels (``.train()``, or
+    an eval forward that records a graph) fp32 copies of the activations that are extra outputs of the native autograd
+    Function, so a loss on them (feature matching, deep supervision, distillation) back-propagates through the native backward.
+    Refused, naming the module: a hook that returns a value (RuntimeError), forward pre-hooks and hooks on the Conv1d /
+    BatchNorm1d / LeakyReLU / Tanh inside a block (NotImplementedError: the kernels fuse them), and module backward hooks on any
+    sub-module (NotImplementedError). Changing a hook's output in place does not change the forward. Without hooks the forward
+    makes exactly the calls it makes otherwise. ``forward_host``, ``forward_host_stream`` and ``enhance_waveforms`` do not go
+    through ``forward`` and fire no hooks.
     """
 
     def __init__(self, n_layers: int = 12, channels_interval: int = 24, precision: str = "fp32_tc",
@@ -409,6 +465,8 @@ class Model(nn.Module):
         # private seam: a callable summing a float64 CUDA view over the ranks in place forces the synchronised BatchNorm path
         # (see _bn_sync_reducer)
         self._bn_allreduce = None
+        # RemovableHandle.next_id at the last hook scan that found no hook (see _forward_hook_plan)
+        self._hook_free_at = None
 
     # ------------------------------------------------------------------------------------------
     # native plumbing
@@ -539,7 +597,10 @@ class Model(nn.Module):
         its own container, as the reference's sub-modules do: in .train() it uses batch statistics and updates its running
         buffers with its own momentum (None: the cumulative factor 1 / num_batches_tracked) and counter; in .eval() it
         normalises by the running statistics and leaves them untouched. fp32 or, with ``train_precision="bf16"`` /
-        ``"tf32"`` / ``"fp16_scaled"``, bf16 / tf32 / fp16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4)."""
+        ``"tf32"`` / ``"fp16_scaled"``, bf16 / tf32 / fp16 tensor-core convolutions (SURVEY §8f row N1, DESIGN §5.4).
+        Forward hooks on the block containers receive the blocks' outputs as extra outputs of the autograd Function, so a loss
+        on them back-propagates into the native backward."""
+        plan = self._forward_hook_plan()
         if any(t.dtype in _HALF for t in self._param_tensors()):
             raise RuntimeError("libwunet_b200 needs contiguous float32 parameters on the input's device: the native training "
                                "step keeps float32 parameters. To train in 16 bits, train the float32 model with "
@@ -577,14 +638,22 @@ class Model(nn.Module):
         if torch.backends.cudnn.deterministic or torch.are_deterministic_algorithms_enabled():
             flags |= _lib.TRAIN_DETERMINISTIC
         blocks_state = None if uniform else ([not tr for tr in training], momenta)
-        y = _NativeTrainStep.apply(self, flags, reducer, blocks_state, self._aligned(x), *params)
+        if plan is None:
+            y = _NativeTrainStep.apply(self, flags, reducer, blocks_state, self._aligned(x), *params)
+        else:
+            export = self._hook_levels(plan)
+            y, *lv = _NativeTrainStepExport.apply(self, flags, reducer, blocks_state, tuple(export), self._aligned(x), *params)
         if not any(training):
+            if plan is not None:
+                self._fire_forward_hooks(plan, x, y, dict(zip(export, lv)))
             return y                                         # running statistics untouched: the folded copies stay valid
         for bn, tr in zip(bns, training):                    # torch.nn.BatchNorm1d bookkeeping
             if tr:
                 bn.num_batches_tracked += 1
         # the kernels updated running_mean / running_var through raw pointers (no _version bump): drop the folded copies
         self._native.invalidate_weights()
+        if plan is not None:
+            self._fire_forward_hooks(plan, x, y, dict(zip(export, lv)))
         return y
 
     def _bn_sync_reducer(self):
@@ -639,14 +708,17 @@ class Model(nn.Module):
         return torch.empty_like(x)
 
     def _forward_native(self, x: torch.Tensor) -> torch.Tensor:
+        plan = self._forward_hook_plan()
         self._check_input(x)
         empty = self._empty_batch(x)
         if empty is not None:
+            if plan is not None:
+                self._fire_forward_hooks(plan, x, empty, {i: self._level_empty(i, x) for i in self._hook_levels(plan)})
             return empty
         if not x.is_cuda:
             raise RuntimeError("wave_u_net_for_speech_enhancement_b200 has no CPU fallback: move the model and the "
                                "input to a CUDA (sm_90a) device")
-        x = self._aligned(x)
+        x_in, x = x, self._aligned(x)
         B, _, T = x.shape
         lib = _lib.load()
         with torch.cuda.device(x.device):
@@ -656,16 +728,124 @@ class Model(nn.Module):
             ws = self._workspace(ctx, B, T, prec, x.device)
             y = torch.empty_like(x)
             stream = torch.cuda.current_stream(x.device).cuda_stream
-            _lib.check(lib.wunet_forward_io(ctx, x.data_ptr(), y.data_ptr(), B, T, prec, _IO_DTYPES[x.dtype], ws.data_ptr(),
-                                            ws.numel(), stream))
+            if plan is None:
+                _lib.check(lib.wunet_forward_io(ctx, x.data_ptr(), y.data_ptr(), B, T, prec, _IO_DTYPES[x.dtype], ws.data_ptr(),
+                                                ws.numel(), stream))
+                return y
+            nb = 2 * self.n_layers + 1
+            levels = {i: self._level_empty(i, x) for i in self._hook_levels(plan)}
+            mask = (ctypes.c_ubyte * nb)(*[1 if i in levels else 0 for i in range(nb)])
+            outs = (ctypes.c_void_p * nb)(*[levels[i].data_ptr() if i in levels else None for i in range(nb)])
+            _lib.check(lib.wunet_forward_export(ctx, x.data_ptr(), y.data_ptr(), B, T, prec, _IO_DTYPES[x.dtype], mask, outs,
+                                                ws.data_ptr(), ws.numel(), stream))
+        self._fire_forward_hooks(plan, x_in, y, levels)
         return y
+
+    # ------------------------------------------------------------------------------------------
+    # forward hooks on the block containers
+    # ------------------------------------------------------------------------------------------
+    def _hook_containers(self):
+        """(name, module, block) of every container whose forward hooks the native forward fires, in the reference's call
+        order (model/unet_basic.py:77-100: an encoder block's ``main`` returns inside the block's own call); block 2n+1 = out."""
+        n = self.n_layers
+        cs = []
+        for i, e in enumerate(self.encoder):
+            cs += [(f"encoder.{i}.main", e.main, i), (f"encoder.{i}", e, i)]
+        cs.append(("middle", self.middle, n))
+        for j, d in enumerate(self.decoder):
+            cs += [(f"decoder.{j}.main", d.main, n + 1 + j), (f"decoder.{j}", d, n + 1 + j)]
+        cs.append(("out", self.out, 2 * n + 1))
+        return cs
+
+    def _forward_hook_plan(self):
+        """None when no forward hook fires on a block container: the forward then makes exactly the calls it makes without
+        hooks. Otherwise the (name, module, block) whose hooks fire, in order. Raises for every hook on a sub-module that the
+        native forward cannot honour, naming the module. A scan that finds nothing is remembered until the next hook handle is
+        created anywhere (every registration creates one), so the hook-free forward pays one comparison."""
+        if getattr(self, "_hook_free_at", None) == RemovableHandle.next_id:
+            return None
+        containers = self._hook_containers()
+        ids = {id(m) for _, m, _ in containers}
+        for name, m in self.named_modules():
+            if m is self:
+                continue
+            what = f"{name} ({type(m).__name__})"
+            if m._backward_hooks or m._backward_pre_hooks:
+                raise NotImplementedError(f"{what} has a module backward hook: the native forward does not call the sub-modules, "
+                                          "so their backward hooks are not supported. Register a tensor hook on the output a "
+                                          "forward hook receives instead.")
+            if m._forward_pre_hooks:
+                raise NotImplementedError(f"{what} has a forward pre-hook: the native forward does not call the sub-modules, so "
+                                          "forward pre-hooks on them are not supported (forward hooks on the block containers are)")
+            if m._forward_hooks and id(m) not in ids:
+                raise NotImplementedError(f"{what} has a forward hook: inside a block the native forward fuses convolution, "
+                                          "BatchNorm and activation, so only forward hooks on encoder[i], encoder[i].main, middle, "
+                                          "decoder[j], decoder[j].main and out are supported")
+        fire = [c for c in containers if c[1]._forward_hooks or _nn_module._global_forward_hooks]
+        if not fire:
+            self._hook_free_at = RemovableHandle.next_id
+            return None
+        return fire
+
+    def _hook_levels(self, plan):
+        """The blocks whose outputs the hooks of ``plan`` receive, as their output or to build their input, ascending."""
+        n = self.n_layers
+        need = set()
+        for _, _, b in plan:
+            if b == 2 * n + 1:
+                need.add(2 * n)                              # out's input: cat([decoder[n-1], x])
+                continue
+            need.add(b)
+            if 0 < b <= n:
+                need.add(b - 1)                              # previous output, decimated
+            elif b > n:
+                need.update((b - 1, 2 * n - b))              # previous output (upsampled) and the skip
+        return sorted(need)
+
+    def _level_empty(self, block: int, x: torch.Tensor) -> torch.Tensor:
+        n, T = self.n_layers, x.shape[-1]
+        L = T >> block if block <= n else T >> (2 * n - block)
+        return torch.empty(x.shape[0], self._blocks()[block][0].out_channels, L, dtype=x.dtype, device=x.device)
+
+    def _fire_forward_hooks(self, plan, x: torch.Tensor, y: torch.Tensor, levels) -> None:
+        """Call the forward hooks of ``plan`` (global ones first, then the module's, as nn.Module.__call__ does) with
+        ``(module, (input,), output)`` or, registered ``with_kwargs``, ``(module, (input,), {}, output)``. ``levels``: block ->
+        output. A decoder block's input is built with torch (F.interpolate and torch.cat on the exported tensors), so its
+        arithmetic is torch's. A hook that returns a value raises: the native forward cannot replace a block's output."""
+        n = self.n_layers
+        inputs = {}
+
+        def block_input(b):
+            if b not in inputs:
+                if b == 0:
+                    inputs[b] = x
+                elif b <= n:
+                    inputs[b] = levels[b - 1][:, :, ::2]
+                elif b <= 2 * n:
+                    up = F.interpolate(levels[b - 1], scale_factor=2, mode="linear", align_corners=True)
+                    inputs[b] = torch.cat([up, levels[2 * n - b]], dim=1)
+                else:
+                    inputs[b] = torch.cat([levels[2 * n], x], dim=1)
+            return inputs[b]
+
+        g_hooks, g_kw = _nn_module._global_forward_hooks, _nn_module._global_forward_hooks_with_kwargs
+        for name, m, b in plan:
+            args, out = (block_input(b),), (y if b == 2 * n + 1 else levels[b])
+            for hid, hook in (*g_hooks.items(), *m._forward_hooks.items()):
+                if hid in m._forward_hooks_with_kwargs or hid in g_kw:
+                    r = hook(m, args, {}, out)
+                else:
+                    r = hook(m, args, out)
+                if r is not None:
+                    raise RuntimeError(f"a forward hook on {name} ({type(m).__name__}) returned a value: the native forward "
+                                       "cannot replace a block's output, so forward hooks must return None")
 
     @torch.no_grad()
     def forward_host(self, x_host: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """End-to-end form of enhancement.py:64-66 (``model(chunk).detach().cpu()``): host tensor in,
         host tensor out; H2D copy, kernels and D2H copy are enqueued by ``wunet_forward_host_io``.
         Parameters must already live on a CUDA device. Pinned tensors give full copy bandwidth. A 16-bit model takes and
-        returns 16-bit tensors (half the copy bytes)."""
+        returns 16-bit tensors (half the copy bytes). Does not go through ``forward``: forward hooks do not fire."""
         self._check_input(x_host)
         if x_host.is_cuda:
             raise RuntimeError("forward_host takes a host tensor")
@@ -696,7 +876,7 @@ class Model(nn.Module):
         yields one output tensor per input batch, in order; H2D copy, kernels and D2H copy of consecutive batches overlap
         (two batches in flight). ``batches``: iterable of pinned ``[B,1,T]`` host tensors (float32, or the dtype of a 16-bit
         model) that must stay alive until their result has been yielded; ``outs``: optional iterable of pinned output
-        tensors of the same dtype."""
+        tensors of the same dtype. Forward hooks do not fire."""
         if self.training or self._bn_any_training():
             raise NotImplementedError("forward_host_stream is eval-only (model and every BatchNorm container in .eval())")
         device = self.out[0].weight.device
