@@ -6,6 +6,8 @@
 Roles: 0 = TMA producer (around its operand-stage waits, after each weight-stage wait), 1 = consumer thread 0 (before / after
 each operand-stage wait), 2 = consumer thread 0 at the start of each epilogue, 4 = upsample producer thread 0 (before / after
 the stage wait, after the hand-off). Times are clock64 cycles from role 1's first stamp.
+Blocks that run the ping-pong form (wunet_tc_pp.cuh) stamp per tile of each consumer warpgroup, role 1 for warpgroup 0 (thread
+0) and role 3 for warpgroup 1 (thread 128): MMA turn taken, MMAs done (= epilogue start), epilogue done; role 2 stays empty.
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

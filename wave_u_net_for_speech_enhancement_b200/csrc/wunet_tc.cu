@@ -974,6 +974,7 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
         cudaFuncSetAttribute(enc0_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         f16::set_smem_attributes();
         wide::set_smem_attributes();
+        pp::set_smem_attributes();
         int dev = 0, sms = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
             st->dev_sms = sms;
@@ -1097,6 +1098,9 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
         const int mode = st->plan_mode == 2 ? 2 : (p.split ? 1 : 0);
         cudaLaunchKernelEx(&cfg, io == IO_F16 ? io_f16::head_kernel(mode, p.mg != 0) : io_bf16::head_kernel(mode, p.mg != 0), P.tmA, P.tmW,
                            P.tmO, p);
+    } else if (pp::selected(p, P.upcat, P.small, io)) {
+        // weight-resident last decoder block: the ping-pong form (bf16 / fp16), one epilogue under the other warpgroup's MMAs
+        cudaLaunchKernelEx(&cfg, pp::conv_kernel(st->plan_mode == 2, p.mg != 0), P.tmA, P.tmW, P.tmO, p);
     } else if (st->plan_mode == 2) {
         // fp16: the twins of the bf16 forms below (no split-precision form, no block 0 over groups of 8)
         cudaLaunchKernelEx(&cfg, f16::conv_kernel(P.pair == 1 ? 9 : (P.upcat ? 5 : 15), P.small, P.upcat && p.mg), P.tmA, P.tmW, P.tmO, p);

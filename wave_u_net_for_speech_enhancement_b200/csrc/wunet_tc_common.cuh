@@ -225,6 +225,18 @@ ConvKernel conv_split_kernel(bool upcat);
 cudaError_t pack_split(const float *w, void *wp, int Cout, int Cin, int K, int Npad, const SplitTable &tab, cudaStream_t stream);
 }  // namespace wide
 
+// The ping-pong form of the large decoder flavour (wunet_tc_pp.cu): each consumer warpgroup owns whole tiles, so that one
+// warpgroup's epilogue runs under the other's MMAs. bf16 and fp16 (plan mode 2), float I/O.
+namespace pp {
+using ConvKernel = f16::ConvKernel;
+void set_smem_attributes();
+ConvKernel conv_kernel(bool fp16, bool mg);
+// whether a block of this plan runs the ping-pong form: the last decoder block (fused head), weight-resident, large flavour, one
+// column split of at most kPpAccCols columns, full-length frames, no split precision, float I/O (io: IoType of the forward).
+// The other resident decoders are bound by their upsample producers, and the form measured no faster there (DESIGN §5.1).
+bool selected(const TcParams &p, bool upcat, bool small, int io);
+}  // namespace pp
+
 // The forms with a 16-bit network input / output (wunet_tc_io.cuh): io_f16 (__half, wunet_tc_io_f16.cu) and io_bf16
 // (__nv_bfloat16, wunet_tc_io_bf16.cu) have the same functions. mode: 0 = bf16, 1 = split precision, 2 = fp16 (tc_* modes).
 #define WUNET_TC_IO_DECLS                                                                                                           \
