@@ -439,6 +439,14 @@ int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int bloc
  * channels_interval up to 64 (a multiple of 8); [14] counts split-precision K-loop positions (three per 64-channel chunk). */
 int wunet_debug_plan_prec(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
                           int precision);
+/* Introspection, host-only: whether conv block `block` runs in 256-row units at that shape and precision (two tiles of one frame
+ * per unit, one per consumer warpgroup, so that each weight stage streamed from L2 serves 256 output rows; blocks whose weights
+ * are not resident in shared memory, DESIGN.md 5.1), and the geometry of that form. The plan of wunet_debug_plan is the same
+ * either way. No reference counterpart. Writes 8 ints, all 0 when the form is not selected:
+ *  [0] selected  [1] input stages  [2] weight stages  [3] taps per weight stage  [4] weight stages per chunk
+ *  [5] dynamic shared memory bytes  [6] grid  [7] units */
+int wunet_debug_plan_m2(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
+                        int precision);
 
 /* Introspection for tests, host-only: the "row-pair" form of one conv block's weights (WUNET_TC_PAIR, DESIGN.md 5.1). A block
  * with `ksize` taps over positions (w = [cout][cin0 + cin1][ksize] fp32, reference layout; model/unet_basic.py:10,23) is the same

@@ -3,6 +3,7 @@ output difference and per-block times, plus the error of both against the fp32 p
 
     timeout 120 python tools/ab_check.py WUNET_TC_GEMM      # dense GEMM over frames for the blocks of <= 16 samples
     timeout 120 python tools/ab_check.py WUNET_TC_MERGE     # merged decoder tail chunk
+    timeout 120 python tools/ab_check.py WUNET_TC_M2        # 256-row units for the streamed-weight blocks
 """
 import os
 import sys

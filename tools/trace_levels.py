@@ -8,6 +8,8 @@ each operand-stage wait), 2 = consumer thread 0 at the start of each epilogue, 4
 the stage wait, after the hand-off). Times are clock64 cycles from role 1's first stamp.
 Blocks that run the ping-pong form (wunet_tc_pp.cuh) stamp per tile of each consumer warpgroup, role 1 for warpgroup 0 (thread
 0) and role 3 for warpgroup 1 (thread 128): MMA turn taken, MMAs done (= epilogue start), epilogue done; role 2 stays empty.
+Blocks that run in 256-row units (wunet_tc_m2.cuh) stamp role 1 before / after each weight-stage wait instead of each
+operand-stage wait; role 2 is the start of each unit's epilogue.
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

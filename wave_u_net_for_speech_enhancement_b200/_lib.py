@@ -79,6 +79,7 @@ def load() -> ctypes.CDLL:
     lib.wunet_profile_read.argtypes = [vp, vp, ci, ctypes.POINTER(ci)]
     lib.wunet_debug_plan.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ci), ci]
     lib.wunet_debug_plan_prec.argtypes = lib.wunet_debug_plan.argtypes + [ci]
+    lib.wunet_debug_plan_m2.argtypes = lib.wunet_debug_plan_prec.argtypes
     lib.wunet_debug_pair_weights.argtypes = [vp, ci, ci, ci, ci, ci, vp]
     lib.wunet_train_workspace_bytes.argtypes = [vp, ci, ci]
     lib.wunet_train_workspace_bytes.restype = cs
@@ -121,7 +122,7 @@ EXPORTED_SYMBOLS = [
     "wunet_frame_clips_f32", "wunet_frame_clips_i16", "wunet_unframe_clips_f32",
     "wunet_wav_info", "wunet_wav_read_f32", "wunet_crop_pairs",
     "wunet_forward_io", "wunet_forward_host_io", "wunet_stream_submit_io", "wunet_frame_clips_f32_io", "wunet_frame_clips_i16_io",
-    "wunet_forward_export", "wunet_train_backward_inject",
+    "wunet_forward_export", "wunet_train_backward_inject", "wunet_debug_plan_m2",
 ]
 
 PLAN_FIELDS = ["L", "Cin0", "Cin1", "Cout", "Npad", "Nh", "nsplit", "Nstride", "MT", "nacc", "packed", "FR", "S", "m_tiles",
@@ -135,6 +136,18 @@ def debug_plan(n_layers: int, channels_interval: int, B: int, T: int, block: int
     buf = (ctypes.c_int * 32)()
     check(load().wunet_debug_plan_prec(n_layers, channels_interval, B, T, block, num_sms, buf, 32, PRECISIONS[precision]))
     return dict(zip(PLAN_FIELDS, [int(v) for v in buf]))
+
+
+M2_FIELDS = ["selected", "na", "nb", "tg", "ngroups", "smem", "grid", "units"]
+
+
+def debug_plan_m2(n_layers: int, channels_interval: int, B: int, T: int, block: int, num_sms: int = 148,
+                  precision: str = "bf16") -> dict:
+    """Whether one conv block runs in 256-row units (two tiles per unit, each weight stage serving both) and the geometry of
+    that form; all zero when it does not (host-only query: works without a GPU)."""
+    buf = (ctypes.c_int * len(M2_FIELDS))()
+    check(load().wunet_debug_plan_m2(n_layers, channels_interval, B, T, block, num_sms, buf, len(M2_FIELDS), PRECISIONS[precision]))
+    return dict(zip(M2_FIELDS, [int(v) for v in buf]))
 
 
 TRAIN_LAYOUT_FIELDS = ["z", "act", "ga", "mean", "invstd", "s1", "s2", "Cin", "Cin0", "Cin1", "Cout", "L", "ksize", "mode",

@@ -7,8 +7,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libwunet_b200.so")
-SOURCES = ["wunet_api.cu", "wunet_fp32.cu", "wunet_tc.cu", "wunet_train.cu", "wunet_train_tc.cu", "wunet_train_tc_f16.cu", "wunet_tc_f16.cu", "wunet_tc_wide.cu", "wunet_tc_pp.cu", "wunet_tc_io_f16.cu", "wunet_tc_io_bf16.cu", "wunet_hooks.cu"]
-HEADERS = ["wunet_common.cuh", "wunet_tc.cuh", "wunet_tc_common.cuh", "wunet_tc_io.cuh", "wunet_tc_kernels.cuh", "wunet_tc_pp.cuh", "wunet_tc_wide.cuh", "wunet_train.cuh", "wunet_train_tc_kernels.cuh", "wunet_wgmma.cuh", os.path.join("..", "..", "include", "wunet_b200.h")]
+SOURCES = ["wunet_api.cu", "wunet_fp32.cu", "wunet_tc.cu", "wunet_train.cu", "wunet_train_tc.cu", "wunet_train_tc_f16.cu", "wunet_tc_f16.cu", "wunet_tc_wide.cu", "wunet_tc_pp.cu", "wunet_tc_m2.cu", "wunet_tc_io_f16.cu", "wunet_tc_io_bf16.cu", "wunet_hooks.cu"]
+HEADERS = ["wunet_common.cuh", "wunet_tc.cuh", "wunet_tc_common.cuh", "wunet_tc_io.cuh", "wunet_tc_kernels.cuh", "wunet_tc_pp.cuh", "wunet_tc_m2.cuh", "wunet_tc_wide.cuh", "wunet_train.cuh", "wunet_train_tc_kernels.cuh", "wunet_wgmma.cuh", os.path.join("..", "..", "include", "wunet_b200.h")]
 
 
 def nvcc_path() -> str:

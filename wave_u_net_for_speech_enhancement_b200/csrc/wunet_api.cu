@@ -803,19 +803,37 @@ int wunet_debug_plan(int n_layers, int channels_interval, int B, int T, int bloc
     return wunet_debug_plan_prec(n_layers, channels_interval, B, T, block, num_sms, fields, capacity, WUNET_PREC_BF16);
 }
 
+// the blocks of a plan query: the channel plan of wunet_create (model/unet_basic.py:38-39, :52-57, :59-62), no weights
+static std::vector<TcBlockSrc> plan_query_blocks(int n, int ci)
+{
+    std::vector<TcBlockSrc> src;
+    for (int i = 0; i < n; ++i) src.push_back(TcBlockSrc{i == 0 ? 1 : i * ci, (i + 1) * ci, 15, nullptr, nullptr, nullptr});
+    src.push_back(TcBlockSrc{n * ci, n * ci, 15, nullptr, nullptr, nullptr});
+    for (int j = 0; j < n; ++j)
+        src.push_back(TcBlockSrc{j == 0 ? 2 * n * ci : (2 * (n - j) + 1) * ci, (n - j) * ci, 5, nullptr, nullptr, nullptr});
+    return src;
+}
+
 int wunet_debug_plan_prec(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
                           int precision)
 {
     if (n_layers < 1 || n_layers > 16 || channels_interval < 1 || B < 1 || T < 1 || (T % (1 << n_layers)) != 0 || num_sms < 1)
         return fail(WUNET_EINVAL, "bad plan query");
     if (tc_mode(precision) < 0) return fail(WUNET_EINVAL, "only the tensor-core precisions (bf16, fp32_tc, fp16) have a tiling plan");
-    const int n = n_layers, ci = channels_interval;
-    std::vector<TcBlockSrc> src;            // same channel plan as wunet_create (model/unet_basic.py:38-39, :52-57, :59-62)
-    for (int i = 0; i < n; ++i) src.push_back(TcBlockSrc{i == 0 ? 1 : i * ci, (i + 1) * ci, 15, nullptr, nullptr, nullptr});
-    src.push_back(TcBlockSrc{n * ci, n * ci, 15, nullptr, nullptr, nullptr});
-    for (int j = 0; j < n; ++j)
-        src.push_back(TcBlockSrc{j == 0 ? 2 * n * ci : (2 * (n - j) + 1) * ci, (n - j) * ci, 5, nullptr, nullptr, nullptr});
-    if (tc_debug_plan(n, ci, src.data(), (int)src.size(), B, T, block, num_sms, fields, capacity, tc_mode(precision)))
+    const std::vector<TcBlockSrc> src = plan_query_blocks(n_layers, channels_interval);
+    if (tc_debug_plan(n_layers, channels_interval, src.data(), (int)src.size(), B, T, block, num_sms, fields, capacity, tc_mode(precision)))
+        return fail(WUNET_EINVAL, "%s", tc_error());
+    return WUNET_OK;
+}
+
+int wunet_debug_plan_m2(int n_layers, int channels_interval, int B, int T, int block, int num_sms, int *fields, int capacity,
+                        int precision)
+{
+    if (n_layers < 1 || n_layers > 16 || channels_interval < 1 || B < 1 || T < 1 || (T % (1 << n_layers)) != 0 || num_sms < 1)
+        return fail(WUNET_EINVAL, "bad plan query");
+    if (tc_mode(precision) < 0) return fail(WUNET_EINVAL, "only the tensor-core precisions (bf16, fp32_tc, fp16) have a tiling plan");
+    const std::vector<TcBlockSrc> src = plan_query_blocks(n_layers, channels_interval);
+    if (tc_debug_plan_m2(n_layers, channels_interval, src.data(), (int)src.size(), B, T, block, num_sms, fields, capacity, tc_mode(precision)))
         return fail(WUNET_EINVAL, "%s", tc_error());
     return WUNET_OK;
 }

@@ -109,6 +109,13 @@ struct TcPlanLevel {
     int kind = 0;                      // reported by wunet_debug_plan in the 'small' field: 2 = dense GEMM over frames (gemm_tc_kernel)
     int pair = 0;                      // row-pair mode: 1 = encoder block (conv_tc_kernel<9, false, ...>), 
                                        // 3 = block 0 over groups of 8 samples (<3, false, ...>)
+    // the 256-row form of a streamed-weight block (wunet_tc_m2.cu; m2::selected): its parameters (operand stages, weight ring,
+    // unit range), its weight map (the stage's tap count differs from the plan's), dynamic shared memory. Not part of the plan
+    // record (wunet_debug_plan); launched for float network I/O.
+    bool m2 = false;
+    TcParams m2p;
+    CUtensorMap tmW2;
+    size_t m2_smem = 0;
 };
 
 // Per-block tiling overrides for tuning sweeps: WUNET_TC_OVR="<block>:key=val,key=val;<block>:..." with keys
@@ -170,6 +177,7 @@ struct TcState {
     bool pf_late = true;               // see TcParams::pf_late; WUNET_TC_PFLATE=0 switches it off (A/B measurements, tests). Since the
                                        // taps of a stage share one wgmma group, the late prefetch is the faster one (dec4 ... dec10, H100)
     bool gemm = true;                  // dense GEMM over frames for blocks of at most 16 samples (WUNET_TC_GEMM=0 switches it off)
+    bool m2 = true;                    // 256-row form of the streamed-weight blocks where m2::selected (WUNET_TC_M2=0 switches it off)
     // row-pair mode (WUNET_TC_PAIR bit 0: first tensor-core encoder block, bit 1: last decoder block + head): virtual blocks with
     // doubled channel counts and Toeplitz-expanded weights (pair_weight), planned on frames of half the length
     int pair_mask = 1;                 // default: block 1 in row-pair mode (enc0 also writes a dense copy of its even rows)
@@ -276,6 +284,7 @@ int tc_set_weights(TcState **pst, int n, int ci, const TcBlockSrc *blocks, int n
         if (const char *xe = getenv("WUNET_TC_MERGE")) st->merge = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_PFLATE")) st->pf_late = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_GEMM")) st->gemm = xe[0] != '0';
+        if (const char *xe = getenv("WUNET_TC_M2")) st->m2 = xe[0] != '0';
         if (const char *xe = getenv("WUNET_TC_L2PROMO")) st->enc_l2promo = atoi(xe);
         if (const char *xe = getenv("WUNET_TC_PAIR")) st->pair_mask = atoi(xe) & 3;
         if (const char *xe = getenv("WUNET_TC_ENC0")) st->enc0_tc = xe[0] == '1';
@@ -838,6 +847,16 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
         if (make_map(st, &P.tmW, sp ? lv.wp_sp : (f16 ? lv.wp16 : lv.wp), ktot, lv.Npad, lv.k, ktot * 2, (uint64_t)lv.Npad * ktot * 2, 64,
                      (uint32_t)p.Nh, (uint32_t)p.tg))
             return -1;
+        P.m2 = false;
+        if (st->m2 && m2::selected(p, lv.k, dec, P.small, P.pair, st->num_sms)) {
+            // 256-row units: the same operands and maps, weight stages of m2p.tg taps
+            m2::geometry(p, lv.k, P.m2p);
+            if (make_map(st, &P.tmW2, f16 ? lv.wp16 : lv.wp, ktot, lv.Npad, lv.k, ktot * 2, (uint64_t)lv.Npad * ktot * 2, 64, (uint32_t)p.Nh,
+                         (uint32_t)P.m2p.tg))
+                return -1;
+            P.m2_smem = smem_total(P.m2p);
+            P.m2 = true;
+        }
     }
     if (getenv("WUNET_TC_DEBUG")) {
         for (int i = pl.enc0_tc ? 0 : 1; i < 2 * n + 1; ++i) {
@@ -851,39 +870,38 @@ static int build_plan(TcState *st, const float *x, float *y, int B, int T, void 
             fprintf(stderr, "[wunet tc] blk %2d L=%5d Cin=%3d+%3d Cout=%3d Nh=%3d x%d MT=%d nacc=%d packed=%d FR=%d res=%d bulk=%d na=%d nb=%d tg=%d smem=%zu tmem=%u tiles=%d grid=%u small=%d per_sm=%d hd=%d ring=%d\n",
                     i, p.L, p.Cin0, p.Cin1, p.Cout, p.Nh, p.nsplit, p.MT, p.nacc, p.packed, p.FR, p.resident, p.bulk_store, p.na, p.nb, p.tg, pl.lv[i].smem, p.tmem_cols,
                     p.m_tiles * p.nsplit, pl.lv[i].grid.x, (int)pl.lv[i].small, pl.lv[i].per_sm, p.hd, p.ps_n);
+            if (pl.lv[i].m2) {
+                const TcParams &q = pl.lv[i].m2p;
+                fprintf(stderr, "[wunet tc]        256-row units=%d na=%d nb=%d tg=%d smem=%zu grid=%d\n", q.tile_end, q.na, q.nb, q.tg,
+                        pl.lv[i].m2_smem, std::min(q.tile_end, st->num_sms));
+            }
         }
     }
     st->plan_ws = ws; st->plan_B = B; st->plan_T = T; st->plan_x = x; st->plan_y = y; st->plan_mode = mode;
     return 0;
 }
 
-int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *f, int cap, int mode)
+// the plan build_plan makes for `block` (host-only, see tc_debug_plan); ks receives the block's tap count
+static int debug_plan_level(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int mode,
+                            TcPlanLevel &P, int &ks)
 {
     const char *e0 = getenv("WUNET_TC_ENC0");
     const bool g8 = mode == 0 && block == 0 && e0 && e0[0] == '1';    // block 0 has a tensor-core plan only in its group-of-8 form (bf16)
     if (nblocks != 2 * n + 1 || (block < 1 && !g8) || block >= nblocks) return tc_fail("block %d out of range (1..%d)", block, 2 * n);
     if (ci % 8 != 0 || ci > 64) return tc_fail("bf16 tensor-core path needs channels_interval %% 8 == 0 and <= 64 (got %d)", ci);
-    if (cap < 32 || !f) return tc_fail("need room for 32 fields");
+    ks = blocks[block].k;
     if (g8) {
         if (blocks[0].k != 15 || blocks[0].cin != 1 || 8 * blocks[0].cout > 256 || T % 8 != 0 || T / 8 < 128) return tc_fail("block 0 has no group-of-8 plan for this shape");
         TcLevel pv;
         pv.cin0 = 8; pv.cin1 = 0; pv.cout = 8 * blocks[0].cout; pv.k = 3; pv.Npad = round_up(pv.cout, 16); pv.Ktot = 64;
-        TcPlanLevel P{};
         const char *ovr = getenv("WUNET_TC_OVR");
-        if (plan_block(pv, 0, n, B, T, num_sms, ovr ? ovr : "", P, false, 0, false, true)) return -1;
-        const TcParams &p = P.p;
-        const int v[32] = {p.L, p.Cin0, p.Cin1, p.Cout, p.Npad, p.Nh, p.nsplit, p.Nstride, p.MT, p.nacc, p.packed, p.FR, p.S, p.m_tiles,
-                           p.nchunks, p.resident, p.bulk_store, p.na, p.nb, p.tg, p.ngroups, (int)p.a_stage_bytes, (int)p.b_stage_bytes,
-                           p.a_tx_bytes, p.rows_used, (int)p.tmem_cols, (int)P.smem, P.threads, P.per_sm, (int)P.grid.x, (int)P.small,
-                           p.tiles_per_frame};
-        for (int k = 0; k < 32; ++k) f[k] = v[k];
-        return 0;
+        ks = pv.k;
+        return plan_block(pv, 0, n, B, T, num_sms, ovr ? ovr : "", P, false, 0, false, true);
     }
     std::vector<TcLevel> levels(nblocks);
     const char *mge = getenv("WUNET_TC_MERGE");
     derive_levels(levels, blocks, nblocks, n, !(mge && mge[0] == '0') && ci <= 32);
     const char *ovr = getenv("WUNET_TC_OVR");
-    TcPlanLevel P{};
     const std::string ovr_s = ovr ? ovr : "";
     const char *ge = getenv("WUNET_TC_GEMM");
     bool planned = false;
@@ -907,6 +925,7 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
                 pv.Ktot = round_up(pv.cin0, 64) + (pv.cin1 ? round_up(pv.cin1, 64) : 0);
                 pv.mg_s = pv.mg_u = 0;
                 if (plan_block(pv, block, n, B, T, num_sms, ovr_s, P, false, 0, true)) return -1;
+                ks = pv.k;
                 planned = true;
             }
         }
@@ -915,12 +934,38 @@ int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, i
                       plan_block_gemm(levels[block], block, n, B, T, num_sms, P)) &&
         plan_block(levels[block], block, n, B, T, num_sms, ovr_s, P, false, 0))
         return -1;
+    return 0;
+}
+
+int tc_debug_plan(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *f, int cap, int mode)
+{
+    if (cap < 32 || !f) return tc_fail("need room for 32 fields");
+    TcPlanLevel P{};
+    int ks = 0;
+    if (debug_plan_level(n, ci, blocks, nblocks, B, T, block, num_sms, mode, P, ks)) return -1;
     const TcParams &p = P.p;
     const int v[32] = {p.L, p.Cin0, p.Cin1, p.Cout, p.Npad, p.Nh, p.nsplit, p.Nstride, p.MT, p.nacc, p.packed, p.FR, p.S, p.m_tiles,
                        p.nchunks, p.resident, p.bulk_store, p.na, p.nb, p.tg, p.ngroups, (int)p.a_stage_bytes, (int)p.b_stage_bytes,
                        p.a_tx_bytes, p.rows_used, (int)p.tmem_cols, (int)P.smem, P.threads, P.per_sm, (int)P.grid.x, P.kind == 2 ? 2 : (int)P.small,
                        p.tiles_per_frame};
     for (int k = 0; k < 32; ++k) f[k] = v[k];
+    return 0;
+}
+
+int tc_debug_plan_m2(int n, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *f, int cap, int mode)
+{
+    if (cap < 8 || !f) return tc_fail("need room for 8 fields");
+    TcPlanLevel P{};
+    int ks = 0;
+    if (debug_plan_level(n, ci, blocks, nblocks, B, T, block, num_sms, mode, P, ks)) return -1;
+    for (int k = 0; k < 8; ++k) f[k] = 0;
+    P.p.head = block == 2 * n ? 1 : 0;                   // as build_plan sets it: the last block carries the fused head
+    const char *me = getenv("WUNET_TC_M2");
+    if (P.is_gemm || (me && me[0] == '0') || !m2::selected(P.p, ks, P.upcat, P.small, P.pair, num_sms)) return 0;
+    TcParams q;
+    m2::geometry(P.p, ks, q);
+    const int v[8] = {1, q.na, q.nb, q.tg, q.ngroups, (int)smem_total(q), std::min(q.tile_end, num_sms), q.tile_end};
+    for (int k = 0; k < 8; ++k) f[k] = v[k];
     return 0;
 }
 
@@ -975,6 +1020,7 @@ static int tc_prepare(TcState *st, const float *x, float *y, int B, int T, void 
         f16::set_smem_attributes();
         wide::set_smem_attributes();
         pp::set_smem_attributes();
+        m2::set_smem_attributes();
         int dev = 0, sms = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
             st->dev_sms = sms;
@@ -1098,6 +1144,15 @@ static int launch_block(TcState *st, int i, int t0, int t1, cudaStream_t stream,
         const int mode = st->plan_mode == 2 ? 2 : (p.split ? 1 : 0);
         cudaLaunchKernelEx(&cfg, io == IO_F16 ? io_f16::head_kernel(mode, p.mg != 0) : io_bf16::head_kernel(mode, p.mg != 0), P.tmA, P.tmW,
                            P.tmO, p);
+    } else if (P.m2 && io == IO_F32 && t1 < 0) {
+        // streamed-weight block in 256-row units (bf16 / fp16): each weight stage serves both consumer warpgroups' tiles
+        TcParams q = P.m2p;
+        q.pf_late = p.pf_late;
+        cfg.gridDim = dim3((unsigned)std::min(q.tile_end - q.tile_begin, st->num_sms), 1, 1);
+        cfg.blockDim = dim3(32 + 32 * (kEpiWarpsLarge + (P.upcat ? m2::kM2ProducerWarps : 0)));
+        cfg.dynamicSmemBytes = P.m2_smem;
+        q.out = p.out;
+        cudaLaunchKernelEx(&cfg, m2::conv_kernel(st->plan_mode == 2, P.upcat, q.mg != 0), P.tmA, P.tmW2, P.tmO, q);
     } else if (pp::selected(p, P.upcat, P.small, io)) {
         // weight-resident last decoder block: the ping-pong form (bf16 / fp16), one epilogue under the other warpgroup's MMAs
         cudaLaunchKernelEx(&cfg, pp::conv_kernel(st->plan_mode == 2, p.mg != 0), P.tmA, P.tmW, P.tmO, p);

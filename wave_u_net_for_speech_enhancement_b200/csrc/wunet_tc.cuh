@@ -39,6 +39,9 @@ void tc_destroy(TcState *st);
 // the split-precision (fp32_tc) plan; mode 2 (fp16) = the bf16 plan
 int tc_debug_plan(int n_layers, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *fields,
                   int capacity, int mode = 0);
+// host-only: whether that block runs in 256-row units (wunet_tc_m2.cu) and their geometry (8 ints, see wunet_debug_plan_m2)
+int tc_debug_plan_m2(int n_layers, int ci, const TcBlockSrc *blocks, int nblocks, int B, int T, int block, int num_sms, int *fields,
+                     int capacity, int mode = 0);
 
 // host-only: row-pair expansion of [Cout][C0+C1][K] weights to [2 Cout][2 (C0+C1)][K'] (tests of the WUNET_TC_PAIR packing)
 int tc_debug_pair_weights(const float *w, int Cout, int C0, int C1, int K, int dec, float *out);

@@ -237,6 +237,29 @@ ConvKernel conv_kernel(bool fp16, bool mg);
 bool selected(const TcParams &p, bool upcat, bool small, int io);
 }  // namespace pp
 
+// The 256-row form of the large flavour for the blocks that stream their weights from L2 (wunet_tc_m2.cu): a work unit is two
+// tiles of one frame, one per consumer warpgroup, so each weight stage serves 256 output rows. bf16 and fp16 (plan mode 2).
+namespace m2 {
+using ConvKernel = f16::ConvKernel;
+// accumulator columns: 2 x 48 fp32 registers per consumer thread. ptxas sizes the register budget for whole warpgroups: 288
+// (encoder) or 384 (decoder) threads per CTA leave 168 registers per thread, 416 only 128. Blocks of 128 columns per CTA keep
+// the 128-row tiles: next to 256-row operand stages their weight stages hold 4 taps, and enc4 measured no faster so.
+constexpr int kM2AccCols = 96;
+constexpr int kM2ProducerWarps = 3;    // upsample producers of the decoder form (conv_tc_kernel: 4, 416 threads per CTA)
+void set_smem_attributes();
+ConvKernel conv_kernel(bool fp16, bool upcat, bool mg);
+// work units (two tiles of one frame and one column split) of a plan; 0 for packed frames or an odd tile count per frame
+int units(const TcParams &p);
+// the block's parameters in this form, from its plan p (ks taps): operand stages of 256 + ks - 1 rows, the weight ring re-fitted
+// next to them (na, tg, ngroups, nb), tile_begin / tile_end counting units; false if it does not fit in shared memory
+bool geometry(const TcParams &p, int ks, TcParams &q);
+// whether a block of this plan runs the form: bf16 / fp16 (no split precision), not the head, the large flavour and no row-pair
+// form (pair == 0), streamed weights, full-length frames with an even tile count, at most kM2AccCols columns per CTA, at
+// least num_sms units (small batches keep the 128-row tiles on every SM), and a geometry that fits.
+// The host also requires float network I/O.
+bool selected(const TcParams &p, int ks, bool upcat, bool small, int pair, int num_sms);
+}  // namespace m2
+
 // The forms with a 16-bit network input / output (wunet_tc_io.cuh): io_f16 (__half, wunet_tc_io_f16.cu) and io_bf16
 // (__nv_bfloat16, wunet_tc_io_bf16.cu) have the same functions. mode: 0 = bf16, 1 = split precision, 2 = fp16 (tc_* modes).
 #define WUNET_TC_IO_DECLS                                                                                                           \
